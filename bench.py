@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — env-steps/sec of the iPLAN rollout-and-learn hot path on B200.
+"""bench.py — env-steps/sec of the iPLAN rollout-and-learn hot path on H100.
 
 One "step" = one pass of the hot path over one batch of synthetic input: a 90-timestep
 rollout of `envs_per_gpu` environments x 5 agents (K1 GAT + K1b behaviour encoder + K1c
@@ -16,6 +16,11 @@ Prints ONE JSON line (rank 0).  `value` = device-resident path, inputs already i
 `e2e` = the same work through the reference-facing numpy API (host buffers in/out every
 timestep); `roofline` = the dominant kernel (K1 GAT step) timed with CUDA events inside the
 timed region; `cpu_baseline` = the oracle port on the host cores (N=1 only).
+`--dump-outputs DIR` writes what the last timed step computed as DIR/<name>.npy (float32; arrays larger than
+DUMP_SAMPLE elements as a fixed, seeded sample of their elements), so that two builds can be compared output for output.
+The inputs are the same in every run with the same arguments, and so are the outputs: the update's cross-block gradient
+sums are added in a fixed order.  (--with-aux adds Behavior_policy.learn and Prediction_policy.learn, whose gradient sums
+still use float atomics: with it the weights agree from run to run only to rounding.)
 """
 import argparse
 import json
@@ -46,24 +51,40 @@ def parse():
                    help="highway = BASELINE configs[2] (headline); microbench = configs[4], the 8192 x 32 x 16 x 128-d GAT + GRU forward")
     p.add_argument("--with-aux", action="store_true",
                    help="also run Behavior_policy.learn and Prediction_policy.learn in every step (run_ippo.py:263-286 order) and report their time")
+    p.add_argument("--dump-outputs", metavar="DIR", default=None,
+                   help="after the timed steps, write the outputs of the last one as DIR/<name>.npy (rank 0)")
     return p.parse_args()
 
 
+DUMP_SAMPLE = 1 << 20        # elements kept per dumped array (4 MB in float32)
+
+
+def dump_outputs(out_dir, arrays):
+    """arrays: name -> tensor.  Each is written flattened as float32; one with more than DUMP_SAMPLE elements is replaced by
+    the elements at DUMP_SAMPLE sorted indices drawn with a fixed seed (the same indices for the same shape)."""
+    import numpy as np
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    for name, t in arrays.items():
+        t = t.detach().reshape(-1)
+        if t.numel() > DUMP_SAMPLE:
+            g = torch.Generator().manual_seed(20240601)
+            idx = torch.randint(0, t.numel(), (DUMP_SAMPLE,), generator=g).sort().values
+            t = t[idx.to(t.device)]
+        np.save(os.path.join(out_dir, name + ".npy"), t.float().cpu().numpy())
+
+
 def peaks():
-    try:
-        with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
-            pk = json.load(f)
-        return dict(hbm=pk["hbm_gbs"], tf_burst=pk["bf16_tflops"], tf_sus=pk.get("bf16_tflops_sustained", pk["bf16_tflops"]),
-                    src="measured")
-    except Exception:
-        return dict(hbm=6650.0, tf_burst=1590.0, tf_sus=1400.0, src="fallback")
+    """NVIDIA's H100 SXM data-sheet figures (dense BF16 tensor rate, HBM3 bandwidth) at a 700 W limit: the yardstick of the
+    roofline fractions, not rates this card has been measured to reach (a lower power limit lowers the attainable clocks)."""
+    return dict(hbm=3350.0, tf_sus=989.0, src="H100 SXM data sheet, dense BF16")
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region, and the card's name and power limit (read-only queries)."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
-         "clocks_event_reasons.sw_power_cap")
+         "clocks_event_reasons.sw_power_cap,power.limit,name")
 
     def __init__(self, gpu_index):
         self.path = tempfile.mktemp(suffix=".csv")
@@ -86,14 +107,15 @@ class ClockSampler:
             self.proc.wait(timeout=5)
         except Exception:
             self.proc.kill()
-        sm, mx, reasons = [], [], set()
+        sm, mx, reasons, plim, name = [], [], set(), None, None
         names = ["hw_slowdown", "hw_thermal_slowdown", "sw_thermal_slowdown", "sw_power_cap"]
         for line in open(self.path):
             f = [x.strip() for x in line.split(",")]
-            if len(f) < 8:
+            if len(f) < 10:
                 continue
             try:
                 sm.append(float(f[1])); mx.append(float(f[2]))
+                plim, name = float(f[8]), f[9]
             except ValueError:
                 continue
             for n, v in zip(names, f[4:8]):
@@ -101,12 +123,12 @@ class ClockSampler:
                     reasons.add(n)
         os.unlink(self.path)
         sm.sort()
-        return {"sm_mhz": sm[len(sm) // 2] if sm else None, "sm_max_mhz": max(mx) if mx else None,
-                "samples": len(sm), "reasons": sorted(reasons)}
+        return {"gpu": name, "power_limit_w": plim, "sm_mhz": sm[len(sm) // 2] if sm else None,
+                "sm_max_mhz": max(mx) if mx else None, "samples": len(sm), "reasons": sorted(reasons)}
 
 
 def gat_algorithmic(B, A, N, o, L, H=32):
-    """Algorithmic FLOPs and HBM bytes of ONE K1 step (DESIGN.md §kernels), split over its two kernels:
+    """Algorithmic FLOPs and HBM bytes of ONE K1 step, split over its two kernels:
     {"recur": (flops, bytes), "attend": (flops, bytes), "step": (flops, bytes)}.  Each node's inputs are counted
     once per kernel that needs them; the kernel-to-kernel logit scratch is not algorithmic traffic."""
     in_dim = o + L
@@ -121,18 +143,6 @@ def gat_algorithmic(B, A, N, o, L, H=32):
     return {"recur": (recur * nodes, nodes * in_dim * 4),
             "attend": (attend * nodes, nodes * (in_dim + 2 * H) * 4),
             "step": ((recur + attend) * nodes, nodes * (in_dim + 2 * H) * 4)}
-
-
-def ncu_traffic(kernel):
-    """dram__bytes_read.sum + dram__bytes_write.sum per launch of `kernel`, from the committed `ncu --set full`
-    summaries (profiles/r2_k1_ncu_summary.json, else round 1's); None if no file names the kernel."""
-    for name in ("r2_k1_ncu_summary.json", "r1_k1_ncu_summary.json"):
-        try:
-            with open(os.path.join(ROOT, "profiles", name)) as f:
-                return json.load(f)[kernel]["dram_bytes_per_launch"]
-        except Exception:
-            continue
-    return None
 
 
 def run_reference(args):
@@ -316,9 +326,9 @@ def run_microbench(args):
                    "envs": MB_ENVS, "envs_per_gpu": envs, "agent_nets": A, "slots": N, "dim": H,
                    "parallelism": f"env-sharded x{world} (forward only: no collective)", "l2": "inputs (2.1 GB per tensor per GPU at N=1) exceed L2"},
         "gpu_launches": launches, "library_gemms_per_step": 9, "clocks": clocks,
-        "roofline": {"kernel": "gat128_recur_kernel (bidirectional 15-step GRU of every ego, W_hh in tensor memory, tcgen05.mma.kind::f16 x3 passes)",
+        "roofline": {"kernel": "gat128_recur_kernel (bidirectional 15-step GRU of every ego, W_hh in shared memory, wgmma m64n16k16 f16 x3 passes)",
                      "bound": "tensor", "achieved": ach, "peak": pk["tf_sus"], "unit": "TFLOP/s", "frac": ach / pk["tf_sus"], "traffic": None,
-                     "peak_source": pk["src"] + " bf16 sustained (MEASURED_PEAKS.json)", "launch_ms": rec_ms,
+                     "peak_source": pk["src"], "launch_ms": rec_ms,
                      "algorithmic_flops_per_launch": f_recur, "share_of_step": rec_ms / ms_per_step,
                      "whole_op": {"algorithmic_flops": f_all, "algorithmic_bytes": b_all, "tflops": f_all / (ms_per_step * 1e-3) / 1e12,
                                   "hbm_frac_of_algorithmic_bytes": b_all / (ms_per_step * 1e-3) / 1e9 / pk["hbm"]}},
@@ -334,6 +344,8 @@ def run_microbench(args):
             out_json["cpu_baseline"] = {"value": v, "unit": "env-steps/s", "cores": R.usable_cpus(), "kind": "reference",
                                         "sample": "the reference's own GAT_Net(128) (oracle/_ref) on 2 nets x 16 envs, scaled in items"}
     print(json.dumps(out_json))
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, {"gat128_out": out})
     if world > 1:
         dist.destroy_process_group()
 
@@ -432,6 +444,16 @@ def main():
     breakdown = {tag: sum(times(tag)) / args.steps for tag in ("gat", "gat_recur", "gat_attend", "ctrl", "beh")}
     aux = {tag: sum(times(tag)) / args.steps for tag in ("aux_behavior_learn", "aux_prediction_learn")} if args.with_aux else None
 
+    if rank == 0 and args.dump_outputs:
+        # the last timed step: the episode its rollout stored and the weights its update produced.  Taken here, before the
+        # e2e leg below runs more steps on the same system.
+        dump = {k: batch[k] for k in ("actions", "reward", "terminated", "attention_latent", "behavior_latent")}
+        dump.update(logp=sysm.runner.last_logp, values=sysm.runner.last_values,
+                    actor_params=sysm.mac.actor_stack.flat, critic_params=sysm.mac.critic_stack.flat)
+        if args.with_aux:
+            dump.update(prediction_params=sysm.prediction.stack.flat, behavior_params=sysm.behavior.stack.flat)
+        dump_outputs(args.dump_outputs, dump)
+
     # ---- e2e: same work through the reference-facing numpy API -----------------------------
     log(f"timed region done: {ms_per_step:.1f} ms/step; e2e leg")
     e2e = None
@@ -459,25 +481,16 @@ def main():
         return
     pk = peaks()
     alg = gat_algorithmic(Bl, a.n_agents, a.max_vehicle_num, a.obs_shape_single, a.latent_dim)
-    impl = int(_lib.lib.iplan_gat_get_impl())
     att_mean = sum(att_ms) / max(1, len(att_ms))
-    fused = impl == 0 and att_mean < 0.02 * max(rec_mean, 1e-9)       # one launch: the second event pair brackets nothing
-    if fused:
-        kname, kkey = "gat_tc5_kernel<fused> (K1 in ONE launch: encode, input projections, 2N GRU chains x N-1 steps on tcgen05/TMEM, hard x soft attention, GRUCell)", "gat_tc5_kernel"
-        flops, hbm_bytes = alg["step"]
-        k_ms, k_all = gat_mean, gat_ms
-    else:
-        kname = ("gat_tc5_kernel (K1 recurrence on tcgen05/TMEM)" if impl == 2 else
-                 "gat_recur_kernel (K1: encode, input projections, 2N GRU chains x N-1 steps, hard-attention logits; mma.sync)")
-        kkey = "gat_tc5_kernel" if impl == 2 else "gat_recur_kernel"
-        flops, hbm_bytes = alg["recur"]
-        k_ms, k_all = rec_mean, rec_ms
+    kname = "gat_recur_kernel (K1: encode, input projections, 2N GRU chains x N-1 steps, hard-attention logits; mma.sync)"
+    flops, hbm_bytes = alg["recur"]
+    k_ms, k_all = rec_mean, rec_ms
     ach_tf = flops / (k_ms * 1e-3) / 1e12 if k_ms > 0 else 0.0
     step_tf = alg["step"][0] / (gat_mean * 1e-3) / 1e12 if gat_mean > 0 else 0.0
-    roofline = {"kernel": kname, "gat_impl": impl,
+    roofline = {"kernel": kname,
                 "bound": "tensor", "achieved": ach_tf, "peak": pk["tf_sus"],
-                "unit": "TFLOP/s", "frac": ach_tf / pk["tf_sus"], "traffic": ncu_traffic(kkey),
-                "peak_source": pk["src"] + " bf16 sustained (MEASURED_PEAKS.json)",
+                "unit": "TFLOP/s", "frac": ach_tf / pk["tf_sus"],
+                "peak_source": pk["src"],
                 "launch_ms": k_ms, "launches_timed": len(k_all),
                 "algorithmic_flops_per_launch": flops, "algorithmic_bytes_per_launch": hbm_bytes,
                 "hbm_achieved_gbs": hbm_bytes / (k_ms * 1e-3) / 1e9 if k_ms > 0 else 0.0,
@@ -485,11 +498,9 @@ def main():
                 "share_of_step": sum(k_all) / ms if ms > 0 else None,
                 "k1_step": {"launch_ms": gat_mean, "attend_ms": att_mean, "tflops": step_tf,
                             "algorithmic_flops": alg["step"][0], "algorithmic_bytes": alg["step"][1],
-                            "share_of_step": sum(gat_ms) / ms if ms > 0 else None,
-                            "traffic_attend": None if fused else ncu_traffic("gat_attend_kernel")},
+                            "share_of_step": sum(gat_ms) / ms if ms > 0 else None},
                 "note": "fp32-accurate products cost 3 f16 MMAs each (hi/lo split): the tensor pipe does 3x the algorithmic FLOPs.  The "
-                        "recurrence is a 54-step serial chain; its gate math (3.75 MUFU + ~25 FP32 instructions per hidden unit and step) "
-                        "bounds the kernel, not the tensor pipe and not HBM (AI ~ 2400 FLOP/B); see DESIGN.md"}
+                        "recurrence is a serial chain of N-1 steps per direction with its gate math between the products"}
     out = {
         "metric": METRIC, "value": value, "unit": "env-steps/s", "n_gpus": world, "steps": args.steps, "warmup": args.warmup,
         "ms_per_step": ms_per_step, "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "f32",

@@ -1,5 +1,5 @@
 /*
- * iplan_b200 — C ABI of the B200-native iPLAN hot path (libiplan_b200.so).
+ * iplan_b200 — C ABI of the CUDA-native iPLAN hot path (libiplan_b200.so), built for sm_90a (H100).
  *
  * The reference (wuxiyang1996/iPLAN) has no FFI layer: its operator boundary is
  * the Python object API of Prediction_policy / Behavior_policy / DcntrlMAC /
@@ -80,20 +80,6 @@ int iplan_gat_step(const float* gat_params, int64_t param_stride,
                    int n_envs, int n_agents, int n_slots, int obs_dim, int latent_dim,
                    void* stream);
 
-/* Which kernels run K1 (nova/GAT_Net.py:41-142):
- *   0  gat_tc5_kernel<fused>   tcgen05.mma + TMEM, one CTA per (2 envs, agent-net): recurrence (both directions),
- *                              attention and GRUCell in ONE launch                                         (default)
- *   1  gat_recur_kernel (mma.sync m16n8k16, one CTA per (env, agent-net, direction)) + gat_attend_kernel  (cross-check)
- *   2  gat_tc5_kernel<recurrence only> + gat_attend_kernel (also what 0 falls back to when n_slots > 57)
- * Same inputs and outputs.  Process-wide; the default can also be chosen with the environment variable IPLAN_GAT_IMPL
- * read at the first call. */
-int iplan_gat_set_impl(int impl);
-int iplan_gat_get_impl(void);
-/* Timing experiments only (IPLAN_GAT_DBG=4): clock64() stamps of one CTA's phase boundaries in the last fused launch. */
-int iplan_gat_debug_clocks(long long* out32);
-/* timing experiments (IPLAN_GAT_DBG=64): per-step event clocks of four warps of one CTA, [4][8 steps][8 events] */
-int iplan_gat_debug_trace(long long* out256);
-
 /* iplan_gat_step with optional cudaEvent_t handles (NULL = skip) recorded on `stream` before the recurrence kernel,
  * between the two kernels and after the attention kernel: per-kernel timing of the dominant kernel inside a running
  * rollout (bench.py's roofline) without a profiler. */
@@ -108,8 +94,8 @@ int iplan_gat_step_ex(const float* gat_params, int64_t param_stride,
  * nova/GAT_Net.py:41-142 with GAT_hidden_dim = attention_dim = 128 and 16 slots per (env, agent-net) "item".  The row x weight
  * products of the op (encode, factored input projections, q|k|v, GRUCell projections) are plain GEMMs that the host runs
  * through a library (iplan_b200/nova/gat128.py); these three kernels are the rest:
- *   iplan_gat128_recur   the bidirectional hard-attention GRU over the 15 neighbours of every ego (:57-97) with W_hh held in
- *                        tensor memory (tcgen05.mma, A operand from TMEM) -> per-edge logit differences
+ *   iplan_gat128_recur   the bidirectional hard-attention GRU over the 15 neighbours of every ego (:57-97) on the warpgroup
+ *                        tensor cores (wgmma, W_hh resident in shared memory) -> per-edge logit differences
  *       P, Q   [2 dirs][A][items][16][384]  ego / neighbour halves of W_ih [enc_i ; enc_j], rows r|z|n, pre-multiplied by the
  *              gate scales (-log2 e for r|z, 2 log2 e for n); Q additionally carries b_ih (+ b_hh for r|z), scaled alike
  *       whh    [A][2][384][128]   bhn [A][2][128] (b_hh of the n gate)   lw [A][2][128] (hard_encoding row 1 - row 0, per direction)
@@ -159,7 +145,7 @@ int iplan_behavior_step_ex(const float* beh_params, int64_t param_stride,
  * dev_* are caller-owned device buffers of the full [B][A][N][*] size (staging for the uploaded arrays; dev_out / dev_new
  * receive the result and stay valid).  Host buffers may be pageable; page-locked ones overlap with the kernels.
  * The GAT noise counter of piece c is counter + c.  chunk_end: NULL (equal pieces) or the n_chunks increasing end indices of
- * the pieces (last = n_envs): K1 runs one CTA per SM, so pieces sized in whole waves with a short last piece (whose copy-out
+ * the pieces (last = n_envs): K1 runs in waves of CTAs over the SMs, so pieces sized in whole waves with a short last piece (whose copy-out
  * nothing overlaps) cost no extra wave. */
 int iplan_gat_latent_update_host(const float* gat_params, int64_t param_stride,
                                  const float* host_hist, float* dev_hist, const float* host_h, float* dev_h,
@@ -174,15 +160,6 @@ int iplan_behavior_latent_update_host(const float* beh_params, int64_t param_str
                                       int n_envs, int n_agents, int n_slots, int obs_dim, int latent_dim, int hist_len, int n_chunks, void* stream);
 /* n device -> host copies on `stream`, then one synchronize (select_actions_ippo returns four small arrays) */
 int iplan_d2h_batch(void* const* dst_host, const void* const* src_dev, const int64_t* bytes, int n, void* stream);
-
-/* Which kernel runs K1b: 0 = behavior_tc5_kernel (tcgen05.mma with both A operands, h and u_w, in tensor memory; chains as
- * TMEM lanes; csrc/behavior_tc5.cu), 1 = behavior_step_kernel (mma.sync m16n8k16, one warp per 16 chains: the cross-check, and
- * the fallback for obs_dim > 8, windows longer than 64 values or hidden-state strides that are not multiples of 4).
- * Returns the previous setting. */
-int iplan_behavior_set_impl(int impl);
-int iplan_behavior_get_impl(void);
-/* timing experiments (IPLAN_BEH_DBG=1): clock64() stamps of one CTA of the last tcgen05 K1b launch, 64 values */
-int iplan_behavior_debug_clocks(long long* out64);
 
 /* ---- K1c: controller step (actor + critic, one timestep) -------------------------
  * replaces DcntrlMAC.select_actions_ippo (controllers/dcntrl_controller.py:27-58):
@@ -288,14 +265,6 @@ int iplan_learner_fc1_forward(const float* actor, int64_t actor_stride, const fl
                               int64_t rows, int n_agents, const float* stat, void* Wh, void* Wl,
                               float* ws, float* cc, float* Z1, void* stream);
 
-/* Same contract, same operands, same results to fp32 rounding; the product runs on the 5th-generation tensor cores
- * (tcgen05.mma, accumulators in TMEM, operand stages filled by TMA — csrc/fc1_tc5.cu).  X must be contiguous over
- * agents (x_stride_agent == rows * ldx); ldx % 8 == 0. */
-int iplan_learner_fc1_forward_tc5(const float* actor, int64_t actor_stride, const float* critic, int64_t critic_stride,
-                                  const void* Xh, const void* Xl, int64_t x_stride_agent, int ldx, int feat_dim,
-                                  int64_t rows, int n_agents, const float* stat, void* Wh, void* Wl,
-                                  float* ws, float* cc, float* Z1, void* stream);
-
 typedef struct {
     const float* actor; const float* critic; int64_t actor_stride, critic_stride;   /* parameters */
     float* g_actor; float* g_critic;                                                /* gradients (train) */
@@ -332,15 +301,6 @@ int iplan_learner_fc1_backward(const float* actor, int64_t actor_stride, const f
                                int64_t rows, int n_agents,
                                const float* dZ1, void* Dh, void* Dl, float* gscale,
                                const float* SM, float* G, void* stream);
-
-/* Same contract and results to fp32 rounding as iplan_learner_fc1_backward; the product runs on tcgen05 tensor cores
- * (csrc/fc1_tc5.cu).  X must be contiguous over agents (x_stride_agent == rows * ldx). */
-int iplan_learner_fc1_backward_tc5(const float* actor, int64_t actor_stride, const float* critic, int64_t critic_stride,
-                                   float* g_actor, float* g_critic,
-                                   const void* Xh, const void* Xl, int64_t x_stride_agent, int ldx, int feat_dim,
-                                   int64_t rows, int n_agents,
-                                   const float* dZ1, void* Dh, void* Dl, float* gscale,
-                                   const float* SM, float* G, void* stream);
 
 /* K2a: GAE backward scan (compute_returns :344-365), raw advantages zeroed where the agent is
  * dead (:273-277) and their moments: moments [A][4] = (sum, sum of squares, count, sum of

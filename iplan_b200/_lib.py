@@ -37,10 +37,6 @@ _SIGNATURES = {
     "iplan_actor_layout": (_i64, [_i, _i, _p]),
     "iplan_critic_layout": (_i64, [_i, _p]),
     "iplan_gat_scratch_floats": (_i64, [_i, _i, _i]),
-    "iplan_gat_set_impl": (_i, [_i]),
-    "iplan_gat_get_impl": (_i, []),
-    "iplan_gat_debug_clocks": (_i, [_p]),
-    "iplan_gat_debug_trace": (_i, [_p]),
     "iplan_gat_step": (_i, [_p, _i64, View, View, View, View, _p, _u64, _u64, _f, _p, _p, _i64,
                             _i, _i, _i, _i, _i, _p]),
     "iplan_gat_step_ex": (_i, [_p, _i64, View, View, View, View, _p, _u64, _u64, _f, _p, _p, _i64,
@@ -48,9 +44,6 @@ _SIGNATURES = {
     "iplan_gat128_recur": (_i, [_p, _p, _p, _p, _p, _p, _i, _i64, _p]),
     "iplan_gat128_attend": (_i, [_p, _p, _p, _p, _p, _u64, _u64, _f, _p, _i, _i64, _p]),
     "iplan_gat128_gates": (_i, [_p, _p, _p, _p, _i64, _p]),
-    "iplan_behavior_set_impl": (_i, [_i]),
-    "iplan_behavior_get_impl": (_i, []),
-    "iplan_behavior_debug_clocks": (_i, [_p]),
     "iplan_behavior_step": (_i, [_p, _i64, View, View, View, View, _f, _i, _i, _i, _i, _i, _i, _p]),
     "iplan_behavior_step_ex": (_i, [_p, _i64, View, _i64, _i, View, View, View, _f, _i, _i, _i, _i, _i, _i, _p]),
     "iplan_gat_latent_update_host": (_i, [_p, _i64, _p, _p, _p, _p, _p, _p, _p, _p, _u64, _u64, _f, _p, _i64, _i, _i, _i, _i, _i, _i, _p, _p]),
@@ -72,12 +65,9 @@ _SIGNATURES = {
     "iplan_learner_row_stats": (_i, [_p, _i64, _i, _i, _i64, _i, _p, _p]),
     "iplan_learner_x_split": (_i, [_p, _i64, _p, _p, _p]),
     "iplan_learner_fc1_forward": (_i, [_p, _i64, _p, _i64, _p, _p, _i64, _i, _i, _i64, _i, _p, _p, _p, _p, _p, _p, _p]),
-    "iplan_learner_fc1_forward_tc5": (_i, [_p, _i64, _p, _i64, _p, _p, _i64, _i, _i, _i64, _i, _p, _p, _p, _p, _p, _p, _p]),
     "iplan_learner_tail": (_i, [_p, _i, _p]),
     "iplan_learner_fc1_backward": (_i, [_p, _i64, _p, _i64, _p, _p, _p, _p, _i64, _i, _i, _i64, _i,
                                         _p, _p, _p, _p, _p, _p, _p]),
-    "iplan_learner_fc1_backward_tc5": (_i, [_p, _i64, _p, _i64, _p, _p, _p, _p, _i64, _i, _i, _i64, _i,
-                                            _p, _p, _p, _p, _p, _p, _p]),
     "iplan_learner_gae": (_i, [_p, _p, _p, _f, _f, _i, _i, _i, _i, _p, _p, _p, _p]),
     "iplan_learner_adv_finalize": (_i, [_p, C.c_double, _p, _i, _p]),
     "iplan_learner_adam": (_i, [_p, _p, _p, _p, _p, _p, _i64, _i64, _i, _f, _f, _f, _f, _i, _f, _f, _p, _i, _p]),
@@ -264,7 +254,7 @@ _sm_count = None
 
 
 def wave_chunks(n_envs, ctas_of):
-    """End indices of the env pieces of a pipelined call of a one-CTA-per-SM kernel (K1); ``ctas_of(envs)`` = its grid size.
+    """End indices of the env pieces of a pipelined call of K1; ``ctas_of(envs)`` = its grid size in units of one SM's resident CTAs.
     Consecutive launches on one stream do not overlap, so every piece pays for a whole last wave.  The pieces therefore hold
     whole waves (never more waves in total than a single launch), the LAST piece is what does not fill the other waves (its
     copy-out is the part of the call nothing overlaps, so it should be short), and the rest is cut in two."""

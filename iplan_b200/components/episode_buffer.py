@@ -7,7 +7,7 @@ preprocess=None, device=...)``, ``update(data, bs, ts, mark_filled)``, ``batch[k
 ``batch[(keys...)]``, ``batch[bs_slice, ts_slice]``, ``max_t_filled()``, ``to()``,
 attributes ``scheme / groups / batch_size / max_seq_length / device / data``.
 
-Layout (DESIGN.md "HBM layout"): when the scheme carries the iPLAN feature keys
+Layout: when the scheme carries the iPLAN feature keys
 ``history``, ``attention_latent`` and ``behavior_latent`` the three are views of ONE packed
 tensor ``packed[A, B, T+1, Fp]`` whose rows are exactly the controller's input vector
 (controllers/dcntrl_controller.py:187-213): per slot ``[history | attention | behaviour]``,

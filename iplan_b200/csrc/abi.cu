@@ -26,6 +26,39 @@ int check_launch(const char* what) {
     }
     return 0;
 }
+DetScratch det_scratch(size_t part_floats, size_t n_counters) {
+    static float* part = nullptr;
+    static unsigned* count = nullptr;
+    static size_t part_cap = 0, count_cap = 0;
+    if (part_floats > part_cap || n_counters > count_cap) {
+        cudaError_t e = cudaDeviceSynchronize();                    // earlier launches may still use the old buffers
+        if (e == cudaSuccess && part_floats > part_cap) {
+            cudaFree(part);
+            part = nullptr; part_cap = 0;
+            e = cudaMalloc(&part, part_floats * sizeof(float));
+            if (e == cudaSuccess) part_cap = part_floats;
+        }
+        if (e == cudaSuccess && n_counters > count_cap) {
+            cudaFree(count);
+            count = nullptr; count_cap = 0;
+            e = cudaMalloc(&count, n_counters * sizeof(unsigned));
+            if (e == cudaSuccess) e = cudaMemset(count, 0, n_counters * sizeof(unsigned));
+            if (e == cudaSuccess) e = cudaDeviceSynchronize();
+            if (e == cudaSuccess) count_cap = n_counters;
+        }
+        if (e != cudaSuccess) {
+            set_error("det_scratch: %zu floats, %zu counters: %s", part_floats, n_counters, cudaGetErrorString(e));
+            return {nullptr, nullptr};
+        }
+    }
+    return {part, count};
+}
+int sm_count() {
+    int dev = 0, n = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0)
+        n = 132;
+    return n;
+}
 
 }  // namespace iplan
 

@@ -2,7 +2,7 @@
 // whole episode batch (reference nova/stable_behavior_policy.py:161-279; SURVEY §8f rank 3).
 //
 // Specified line by line by oracle/iplan_oracle.py::behavior_learn_agent (pinned to a recorded run of the reference);
-// checked on a B200 against that run by tools/check_beh_learn.py (losses 2e-7, gradients <= 1e-5 relative).
+// checked against that run by tools/check_beh_learn.py.
 //
 // Per agent-net and episode b the N slots are independent chains through the n_pos = T - 1 - W window positions:
 //   pred_j, dh_{j+1} = Decoder([window_j | latent_j] ; dh_j)       W-step GRU(64), tanh, dropout, linear   (behavior_net.py:40-72)

@@ -18,7 +18,7 @@
 //     forward + backward (loss, decoder gradients, d loss / d latent_j) -> encoder backward.  Three launches.
 //
 // Plain fp32 FFMA on purpose: the legacy mma.sync path would need three f16 passes per product for fp32 accuracy
-// (2.5 x the FMA peak at best), a tcgen05 version is the next step (DESIGN.md §8).
+// (2.5 x the FMA peak at best), a tensor-core version is the next step.
 #include "common.cuh"
 
 namespace iplan {

@@ -1,4 +1,4 @@
-// Launch arguments shared by the two K1b kernels (behavior_step.cu: mma.sync; behavior_tc5.cu: tcgen05).
+// Launch arguments of the K1b kernel (behavior_step.cu).
 #pragma once
 #include "common.cuh"
 
@@ -12,9 +12,5 @@ struct BehArgs {
     int64_t win_step;      // 0: window rows are contiguous ([hist_len][obs_dim] per node); else element stride between rows
     int win_pad;           // (win_step != 0) leading window rows that are zero padding; window.ptr = the first real row
 };
-
-// tcgen05 kernel (behavior_tc5.cu); returns 0 / error
-int launch_behavior_tc5(const BehArgs& a, int n_agents, cudaStream_t st);
-bool behavior_tc5_supports(const BehArgs& a);
 
 }  // namespace iplan

@@ -20,8 +20,6 @@
 #include "common.cuh"
 #include "behavior_common.cuh"
 
-#define IPLAN_BEH_IMPL_DEFAULT 0
-
 namespace iplan {
 
 constexpr int E = IPLAN_HID;       // encoder_rnn_dim
@@ -323,19 +321,6 @@ __global__ void __launch_bounds__(BEH_THREADS, 2) behavior_step_kernel(BehArgs a
 
 }  // namespace iplan
 
-// 0 = behavior_tc5_kernel (tcgen05 / TMEM, csrc/behavior_tc5.cu), 1 = behavior_step_kernel (mma.sync, this file: the
-// cross-check, and the fallback for shapes the tcgen05 kernel does not take).  IPLAN_BEH_IMPL overrides the default at start-up.
-static int g_beh_impl = -1;
-static int beh_impl() {
-    if (g_beh_impl < 0) {
-        const char* ev = getenv("IPLAN_BEH_IMPL");
-        g_beh_impl = ev ? (atoi(ev) != 0) : IPLAN_BEH_IMPL_DEFAULT;
-    }
-    return g_beh_impl;
-}
-extern "C" int iplan_behavior_set_impl(int impl) { const int old = beh_impl(); if (impl == 0 || impl == 1) g_beh_impl = impl; return old; }
-extern "C" int iplan_behavior_get_impl(void) { return beh_impl(); }
-
 extern "C" int iplan_behavior_step(const float* beh_params, int64_t param_stride,
                                    iplan_view window, iplan_view hid_io, iplan_view lat_prev, iplan_view lat_out,
                                    float soft_coef,
@@ -366,7 +351,6 @@ extern "C" int iplan_behavior_step_ex(const float* beh_params, int64_t param_str
     a.coef = soft_coef;
     a.n_envs = n_envs; a.n_slots = n_slots; a.obs_dim = obs_dim; a.latent_dim = latent_dim; a.hist_len = hist_len;
     a.win_step = win_stride_step; a.win_pad = win_stride_step ? win_pad : 0;
-    if (beh_impl() == 0 && behavior_tc5_supports(a)) return launch_behavior_tc5(a, n_agents, (cudaStream_t)stream);
     const size_t smem = sizeof(BehSmem);
     static bool configured = false;
     if (!configured) {

@@ -1,4 +1,4 @@
-// Shared device helpers for the iPLAN sm_100a kernels.
+// Shared device helpers for the iPLAN sm_90a kernels.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -14,6 +14,17 @@ namespace iplan {
 void set_error(const char* fmt, ...);
 void count_launch(int n = 1);
 int  check_launch(const char* what);
+int  sm_count();                 // multiprocessors of the current device (grid sizing)
+
+// ---- deterministic cross-CTA sums ---------------------------------------------------------------
+// Float atomics from several CTAs add in the order the CTAs happen to finish, so the rounding of the result changes from run
+// to run.  Where several CTAs contribute to one sum, each CTA of the group instead stores its partial into its own slot of
+// `part` and arrives at the group's counter; the last CTA to arrive adds the slots in slot order (det_last_arrival), which
+// gives the same bits in every run.  det_scratch() returns library-owned device buffers of at least the given sizes, with
+// every counter zero between launches (the reducing CTA resets its counter); it grows them on demand, synchronising the
+// device when it does.  Launches that use it must be ordered on one stream.
+struct DetScratch { float* part; unsigned* count; };
+DetScratch det_scratch(size_t part_floats, size_t n_counters);      // part == NULL on failure (error text set)
 
 #define IPLAN_REQUIRE(cond, ...)                 \
     do {                                         \
@@ -94,6 +105,22 @@ __host__ __device__ inline TrunkLayout trunk_layout(int feat_dim, int head_out, 
 }
 
 #ifdef __CUDACC__
+// Called by every thread of the CTA after it stored its share of the CTA's partial; true in the CTA that reduces the group
+// (the partials of the others are then visible to it; read them with __ldcg).
+__device__ __forceinline__ bool det_last_arrival(unsigned* counter, unsigned members) {
+    __shared__ unsigned s_last;
+    __threadfence();
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        const unsigned prev = atomicAdd(counter, 1u);
+        s_last = prev == members - 1;
+        if (s_last) atomicExch(counter, 0u);
+    }
+    __syncthreads();
+    if (s_last) __threadfence();
+    return s_last != 0;
+}
+
 // ---- math ---------------------------------------------------------------------------
 __device__ __forceinline__ float sigmoidf_acc(float x) { return 1.0f / (1.0f + expf(-x)); }
 __device__ __forceinline__ float tanhf_acc(float x) { return tanhf(x); }

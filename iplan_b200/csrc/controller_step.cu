@@ -20,7 +20,7 @@ namespace iplan {
 constexpr int R = IPLAN_RNN;            // 64
 constexpr int CTRL_THREADS = 256;
 constexpr int CTRL_WARPS = CTRL_THREADS / 32;
-constexpr int CTRL_ROWS = 18;            // 512 envs -> 29 row groups x 5 agents = 145 CTAs: one wave on 148 SMs
+constexpr int CTRL_ROWS = 18;            // at the Highway feature width 18 rows are what fits in 227 KB of shared memory
 constexpr int CTRL_MT = (CTRL_ROWS + 15) / 16;   // MMA m-tiles per CTA
 constexpr float LN_EPS = 1e-5f;
 

@@ -255,7 +255,8 @@ constexpr size_t BW_SMEM = (size_t)F1_STAGES * BW_STAGE * sizeof(__half);
 __global__ void __launch_bounds__(F1_THREADS, 1) fc1_bwd_mma_kernel(
     const __half* __restrict__ Xh, const __half* __restrict__ Xl, int64_t x_sa, int ldx, int rows, int rows_per_chunk,
     const __half* __restrict__ Dh, const __half* __restrict__ Dl, const float* __restrict__ gscale,
-    float* __restrict__ G /* [A][128][ldx] */) {
+    float* __restrict__ G /* [A][128][ldx] */, float* __restrict__ part /* [A][f tiles][chunks][128][F1_BN] */,
+    unsigned* __restrict__ count /* [A][f tiles] */) {
     extern __shared__ __align__(16) __half smem_h[];
     const int a = blockIdx.z, f0 = blockIdx.x * F1_BN;
     const int r0 = blockIdx.y * rows_per_chunk, r1 = min(rows, r0 + rows_per_chunk);
@@ -348,21 +349,32 @@ __global__ void __launch_bounds__(F1_THREADS, 1) fc1_bwd_mma_kernel(
             }
     }
     cp_async_wait<0>();
+    // this chunk's 128 x F1_BN tile of G into its slot; the last chunk of the tile to finish adds the slots in chunk order
     const float unscale = gscale[a];
     const int gq = lane >> 2, tq = lane & 3;
+    const int64_t group = (int64_t)a * gridDim.x + blockIdx.x;
+    float* slot = part + (group * gridDim.y + blockIdx.y) * (128 * F1_BN);
 #pragma unroll
     for (int i = 0; i < 2; ++i)
 #pragma unroll
         for (int hrow = 0; hrow < 2; ++hrow) {
             const int kk = wm * 32 + i * 16 + gq + hrow * 8;
-            float* gr = G + ((int64_t)a * 128 + kk) * ldx;
 #pragma unroll
             for (int j = 0; j < 8; ++j) {
-                const int f = f0 + wn * 64 + j * 8 + 2 * tq;
-                if (f < ldx) atomicAdd(gr + f, acc[i][j][2 * hrow] * unscale);
-                if (f + 1 < ldx) atomicAdd(gr + f + 1, acc[i][j][2 * hrow + 1] * unscale);
+                const int fl = wn * 64 + j * 8 + 2 * tq;
+                *reinterpret_cast<float2*>(slot + kk * F1_BN + fl) =
+                    make_float2(acc[i][j][2 * hrow] * unscale, acc[i][j][2 * hrow + 1] * unscale);
             }
         }
+    if (!det_last_arrival(count + group, gridDim.y)) return;
+    const float* slots = part + group * gridDim.y * (128 * F1_BN);
+    for (int idx = tid; idx < 128 * F1_BN; idx += F1_THREADS) {
+        const int kk = idx / F1_BN, f = f0 + idx % F1_BN;
+        if (f >= ldx) continue;
+        float s = 0.0f;
+        for (unsigned c = 0; c < gridDim.y; ++c) s += __ldcg(slots + (int64_t)c * (128 * F1_BN) + idx);
+        G[((int64_t)a * 128 + kk) * ldx + f] += s;
+    }
 }
 
 }  // namespace iplan
@@ -371,7 +383,7 @@ using namespace iplan;
 
 extern "C" int iplan_learner_x_split(const float* X, int64_t n_elems, void* Xh, void* Xl, void* stream) {
     IPLAN_REQUIRE(X && Xh && Xl && n_elems > 0 && n_elems % 2 == 0, "x_split: bad arguments");
-    x_split_kernel<<<148 * 8, 256, 0, (cudaStream_t)stream>>>(X, n_elems / 2, (__half2*)Xh, (__half2*)Xl);
+    x_split_kernel<<<sm_count() * 8, 256, 0, (cudaStream_t)stream>>>(X, n_elems / 2, (__half2*)Xh, (__half2*)Xl);
     count_launch();
     return check_launch("x_split");
 }
@@ -402,33 +414,6 @@ extern "C" int iplan_learner_fc1_forward(const float* actor, int64_t actor_strid
 // defined in learner.cu
 namespace iplan { int launch_fc1_grad_finish(const float*, int64_t, const float*, int64_t, float*, float*, int, const float*, int, const float*, int, cudaStream_t); }
 
-namespace iplan {
-int launch_fc1_fwd_tc5(const void* Xh, const void* Xl, int ldx, int64_t rows, int n_agents, const void* Wh, const void* Wl,
-                       const float* ws, const float* cc, const float* stat, float* Z1, cudaStream_t st);   // fc1_tc5.cu
-int launch_fc1_bwd_tc5(const void* Xh, const void* Xl, int ldx, int64_t rows, int n_agents, const void* Dh, const void* Dl,
-                       const float* unscale, float* G, cudaStream_t st);                                     // fc1_tc5.cu
-}
-
-// Same contract as iplan_learner_fc1_forward; the product runs on tcgen05 tensor cores with TMEM accumulators and
-// TMA-fed operand stages (fc1_tc5.cu).  Requires X contiguous over agents (x_stride_agent == rows * ldx).
-extern "C" int iplan_learner_fc1_forward_tc5(const float* actor, int64_t actor_stride, const float* critic, int64_t critic_stride,
-                                             const void* Xh, const void* Xl, int64_t x_stride_agent, int ldx, int feat_dim,
-                                             int64_t rows, int n_agents, const float* stat, void* Wh, void* Wl,
-                                             float* ws, float* cc, float* Z1, void* stream) {
-    IPLAN_REQUIRE(actor && critic && Xh && Xl && stat && Wh && Wl && ws && cc && Z1, "fc1_forward_tc5: null pointer");
-    IPLAN_REQUIRE(ldx % 8 == 0 && ldx >= feat_dim, "fc1_forward_tc5: ldx must be a multiple of 8 and >= feat_dim");
-    IPLAN_REQUIRE(rows > 0 && (int64_t)n_agents * rows < (1ll << 31), "fc1_forward_tc5: bad row count");
-    IPLAN_REQUIRE(x_stride_agent == rows * (int64_t)ldx, "fc1_forward_tc5: X must be contiguous over agents");
-    IPLAN_REQUIRE(((uintptr_t)Xh | (uintptr_t)Xl | (uintptr_t)Wh | (uintptr_t)Wl) % 16 == 0, "fc1_forward_tc5: operands must be 16-byte aligned");
-    cudaStream_t st = (cudaStream_t)stream;
-    NetP P{actor, critic, actor_stride, critic_stride};
-    fc1_prep16_kernel<<<dim3(128, n_agents), 256, 0, st>>>(P, feat_dim, ldx, (__half*)Wh, (__half*)Wl, ws, cc);
-    int rc = launch_fc1_fwd_tc5(Xh, Xl, ldx, rows, n_agents, Wh, Wl, ws, cc, stat, Z1, st);
-    if (rc) return rc;
-    count_launch(2);
-    return check_launch("fc1_forward_tc5");
-}
-
 extern "C" int iplan_learner_fc1_backward(const float* actor, int64_t actor_stride, const float* critic, int64_t critic_stride,
                                           float* g_actor, float* g_critic,
                                           const void* Xh, const void* Xl, int64_t x_stride_agent, int ldx, int feat_dim,
@@ -450,42 +435,16 @@ extern "C" int iplan_learner_fc1_backward(const float* actor, int64_t actor_stri
     unsigned* amax = reinterpret_cast<unsigned*>(gscale);          // [A] max bits | [A] 2^-e
     float* unscale = gscale + n_agents;
     const int64_t npa = rows * 128;
-    absmax_kernel<<<dim3(148, n_agents), 256, 0, st>>>(dZ1, npa, amax);
-    dz_split_kernel<<<dim3(148 * 2, n_agents), 256, 0, st>>>(dZ1, npa, amax, (__half*)Dh, (__half*)Dl, unscale);
+    absmax_kernel<<<dim3(sm_count(), n_agents), 256, 0, st>>>(dZ1, npa, amax);
+    dz_split_kernel<<<dim3(sm_count() * 2, n_agents), 256, 0, st>>>(dZ1, npa, amax, (__half*)Dh, (__half*)Dl, unscale);
     const int chunk = 2048;
     dim3 grid((unsigned)((ldx + F1_BN - 1) / F1_BN), (unsigned)((rows + chunk - 1) / chunk), n_agents);
+    const DetScratch ds = det_scratch((size_t)grid.x * grid.y * grid.z * 128 * F1_BN, (size_t)grid.x * grid.z);
+    if (!ds.part) return -1;                                       // det_scratch set the error text
     fc1_bwd_mma_kernel<<<grid, F1_THREADS, BW_SMEM, st>>>((const __half*)Xh, (const __half*)Xl, x_stride_agent, ldx, (int)rows, chunk,
-                                                           (const __half*)Dh, (const __half*)Dl, unscale, G);
+                                                           (const __half*)Dh, (const __half*)Dl, unscale, G, ds.part, ds.count);
     count_launch(3);
     int rc = check_launch("fc1_backward");
-    if (rc) return rc;
-    return launch_fc1_grad_finish(actor, actor_stride, critic, critic_stride, g_actor, g_critic, feat_dim, G, ldx, SM, n_agents, st);
-}
-
-// Same contract as iplan_learner_fc1_backward; the product G = dZ1^T X runs on tcgen05 (fc1_tc5.cu).
-// Requires X contiguous over agents (x_stride_agent == rows * ldx).
-extern "C" int iplan_learner_fc1_backward_tc5(const float* actor, int64_t actor_stride, const float* critic, int64_t critic_stride,
-                                              float* g_actor, float* g_critic,
-                                              const void* Xh, const void* Xl, int64_t x_stride_agent, int ldx, int feat_dim,
-                                              int64_t rows, int n_agents,
-                                              const float* dZ1, void* Dh, void* Dl, float* gscale /* [A][2] */,
-                                              const float* SM, float* G, void* stream) {
-    IPLAN_REQUIRE(actor && critic && g_actor && g_critic && Xh && Xl && dZ1 && Dh && Dl && gscale && SM && G, "fc1_backward_tc5: null pointer");
-    IPLAN_REQUIRE(ldx % 8 == 0 && rows > 0 && rows < (1ll << 31), "fc1_backward_tc5: bad sizes");
-    IPLAN_REQUIRE(x_stride_agent == rows * (int64_t)ldx, "fc1_backward_tc5: X must be contiguous over agents");
-    cudaStream_t st = (cudaStream_t)stream;
-    cudaError_t e = cudaMemsetAsync(G, 0, sizeof(float) * (size_t)n_agents * 128 * ldx, st);
-    if (e == cudaSuccess) e = cudaMemsetAsync(gscale, 0, sizeof(float) * 2 * n_agents, st);
-    if (e != cudaSuccess) { set_error("fc1_backward_tc5: memset: %s", cudaGetErrorString(e)); return (int)e; }
-    unsigned* amax = reinterpret_cast<unsigned*>(gscale);          // [A] max bits | [A] 2^-e
-    float* unscale = gscale + n_agents;
-    const int64_t npa = rows * 128;
-    absmax_kernel<<<dim3(148, n_agents), 256, 0, st>>>(dZ1, npa, amax);
-    dz_split_kernel<<<dim3(148 * 2, n_agents), 256, 0, st>>>(dZ1, npa, amax, (__half*)Dh, (__half*)Dl, unscale);
-    int rc = launch_fc1_bwd_tc5(Xh, Xl, ldx, rows, n_agents, Dh, Dl, unscale, G, st);
-    if (rc) return rc;
-    count_launch(3);
-    rc = check_launch("fc1_backward_tc5");
     if (rc) return rc;
     return launch_fc1_grad_finish(actor, actor_stride, critic, critic_stride, g_actor, g_critic, feat_dim, G, ldx, SM, n_agents, st);
 }

@@ -1,43 +1,39 @@
-// GAT_Net.forward at GAT_hidden_dim = attention_dim = 128 (BASELINE.json configs[4]: the synthetic GAT + GRU microbench,
-// 8192 envs x 32 agent-nets x 16 slots x 128-d; the op is reference nova/GAT_Net.py:41-142 with wider layers).
+// GAT_Net.forward at GAT_hidden_dim = attention_dim = 128 (the synthetic GAT + GRU microbench, 8192 envs x 32 agent-nets x
+// 16 slots x 128-d; the op is reference nova/GAT_Net.py:41-142 with wider layers).
 //
-// At H = 128 the hidden-state weights of one direction (384 x 128, as f16 hi + lo: 196 KB) no longer fit in shared
-// memory next to anything else, and one chain's ego projection is 384 values.  So the product is turned around:
+// At H = 128 one chain's ego projection is 384 values and the hidden-state weights of one direction (384 x 128) are 96 KB
+// per f16 part.  So the product is turned around:
 //
-//     D^T[gate row (384 = 3 M-tiles of 128)][chain (N = 16 = the egos of one item)] = W_hh[384 x 128] . h^T[128 x 16]
+//     D^T[gate row (384)][chain (N = 16 = the egos of one item)] = W_hh[384 x 128] . h^T[128 x 16]
 //
-//   A = W_hh lives in TENSOR MEMORY for the lifetime of the CTA (tcgen05.mma with the A operand in TMEM: 3 M-tiles x
-//       (64 hi + 64 lo) 32-bit columns = 384 of the 512 columns), written once with tcgen05.st;
-//   B = h^T of one item, a K-major SWIZZLE_128B tile [16 chains][128 hi | 128 lo] f16 (8 KB) rewritten by the gate warps every step;
-//   D = 3 x 16 fp32 columns per item; two items are in flight per CTA (two groups of four warps, 48 columns each), so
-//       one group's gate math overlaps the other group's product.
-// A thread is one HIDDEN UNIT u (TMEM lane u of every M-tile holds the r, z and n pre-activations of unit u) for the 16
-// chains of its group's item: it adds P (registers, constant over the 15 steps) and Q (shared memory), applies the gates
-// (packed fp32 pairs over adjacent chains, ex2 + shared rcp as in K1), keeps h in fp32 registers and writes its f16 hi / lo
-// halves into the operand tile.  The per-step hard-attention logit (a sum over the 128 units = over the 128 threads of the
-// group) is a warp butterfly + a 4-warp exchange through shared memory.
+// and runs on the Hopper warpgroup tensor cores (wgmma.mma_async m64n16k16, f16 inputs, fp32 accumulators in registers):
+//   A = W_hh of this (agent-net, direction), f16 hi + lo parts (192 KB), written once per CTA into shared memory as K-major
+//       SWIZZLE_128B tiles of [64 gate rows][64 k];
+//   B = h^T of the current item, a K-major SWIZZLE_128B tile [16 chains][128 hi | 128 lo] f16 (8 KB), double buffered:
+//       step s reads one buffer while the gate math writes h_{s+1} into the other, so one CTA barrier per step suffices.
+// fp32 accuracy comes from the hi / lo split: hi*hi + hi*lo + lo*hi (three passes of 8 k-blocks; lo*lo < 2^-22 relative).
+// Warpgroup w owns hidden units 64 w .. 64 w + 63 of all three gates (M-tiles r, z, n), so the r, z and n pre-activations of
+// a (unit, chain) land in the same thread: two units x four chains per thread.  It adds P (registers, constant over the 15
+// steps) and Q (read from L2 while the product runs), applies the gates (ex2 + shared rcp as in K1), keeps h in fp32
+// registers and writes its f16 hi / lo halves into the next operand tile.  The per-step hard-attention logit (a sum over
+// the 128 units) is a butterfly over the 8 rows of a warp fragment + an 8-warp exchange through shared memory.
 //
 // The GEMM-shaped parts of the op (encode, the factored input projections P | Q, q | k | v, the GRUCell projections) are
 // plain row x weight products over all 4.2 M slots: the host side runs them as library GEMMs (cuBLAS fp32 through
 // torch.matmul, iplan_b200/nova/gat128.py); this file holds the recurrence, the attention and the GRUCell gate kernels.
-#include <stdlib.h>
-
 #include "common.cuh"
 #include "gat_common.cuh"
-#include "tc5.cuh"
 
 namespace iplan {
 
 constexpr int HB = 128, G3B = 3 * HB, NB = 16, STEPS = NB - 1;
-constexpr int G8_THREADS = 256;                      // two groups of four warps; thread = (group, hidden unit)
+constexpr int G8_THREADS = 256;                      // two warpgroups; warpgroup w = hidden units 64 w .. 64 w + 63
+constexpr int G8_WTILE = 64 * 128;                   // one [64 rows][64 k] f16 operand tile (rows of 128 B)
+constexpr int G8_OFF_W = 0;                          // W_hh tiles [gate 3][warpgroup 2][k half 2][hi | lo]
 constexpr int G8_BT_BYTES = 4 * NB * 128;            // h^T operand tile: 4 sub-tiles (hi k<64, hi k>=64, lo, lo) of [16 rows][128 B]
-constexpr int G8_Q_BYTES = NB * G3B * 4;             // one item's Q table
-constexpr int G8_OFF_BT = 0;                         // 2 groups
-constexpr int G8_OFF_Q = 2 * G8_BT_BYTES;            // 2 groups x 2 buffers
-constexpr int G8_OFF_PL = G8_OFF_Q + 4 * G8_Q_BYTES; // logit exchange [2 groups][2 parities][4 warps][16]
-constexpr int G8_OFF_BAR = G8_OFF_PL + 2 * 2 * 4 * NB * 4;
-constexpr size_t G8_SMEM = G8_OFF_BAR + 64 + 1024;
-constexpr int G8_D_COL = 384;                        // accumulators: group g at columns 384 + 48 g (r | z | n, 16 chains each)
+constexpr int G8_OFF_BT = G8_OFF_W + 24 * G8_WTILE;  // 2 buffers
+constexpr int G8_OFF_PL = G8_OFF_BT + 2 * G8_BT_BYTES;   // logit exchange [2 parities][8 warps][16 chains]
+constexpr size_t G8_SMEM = G8_OFF_PL + 2 * 8 * NB * 4 + 1024;   // + alignment of the base to 1024 B (swizzle atoms)
 
 struct Gat128Args {
     const float* P; const float* Q;                  // [2 dirs][A][items][16][384] gate-scaled ego / neighbour projections (+ biases in Q)
@@ -48,220 +44,213 @@ struct Gat128Args {
     int n_agents; int64_t n_items; int items_per_cta;
 };
 
-__device__ __forceinline__ void tc5_st16(uint32_t taddr, const uint32_t (&v)[16]) {
-    asm volatile("tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16};"
-                 ::"r"(taddr), "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]),
-                   "r"(v[8]), "r"(v[9]), "r"(v[10]), "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15]) : "memory");
-}
-__device__ __forceinline__ void tc5_wait_ld16x3(float (&a)[16], float (&b)[16], float (&c)[16]) {
-    asm volatile("tcgen05.wait::ld.sync.aligned;"
-                 : "+f"(a[0]), "+f"(a[1]), "+f"(a[2]), "+f"(a[3]), "+f"(a[4]), "+f"(a[5]), "+f"(a[6]), "+f"(a[7]),
-                   "+f"(a[8]), "+f"(a[9]), "+f"(a[10]), "+f"(a[11]), "+f"(a[12]), "+f"(a[13]), "+f"(a[14]), "+f"(a[15]),
-                   "+f"(b[0]), "+f"(b[1]), "+f"(b[2]), "+f"(b[3]), "+f"(b[4]), "+f"(b[5]), "+f"(b[6]), "+f"(b[7]),
-                   "+f"(b[8]), "+f"(b[9]), "+f"(b[10]), "+f"(b[11]), "+f"(b[12]), "+f"(b[13]), "+f"(b[14]), "+f"(b[15]),
-                   "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3]), "+f"(c[4]), "+f"(c[5]), "+f"(c[6]), "+f"(c[7]),
-                   "+f"(c[8]), "+f"(c[9]), "+f"(c[10]), "+f"(c[11]), "+f"(c[12]), "+f"(c[13]), "+f"(c[14]), "+f"(c[15])
-                 :: "memory");
-}
+__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void sts16(uint32_t addr, uint16_t v) {
     asm volatile("st.shared.u16 [%0], %1;" ::"r"(addr), "h"(v) : "memory");
 }
-__device__ __forceinline__ void cp_async16(uint32_t dst, const void* src) {
-    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(dst), "l"(src) : "memory");
+__device__ __forceinline__ void sts128(uint32_t addr, uint32_t x, uint32_t y, uint32_t z, uint32_t w) {
+    asm volatile("st.shared.v4.u32 [%0], {%1,%2,%3,%4};" ::"r"(addr), "r"(x), "r"(y), "r"(z), "r"(w) : "memory");
+}
+// generic-proxy writes to shared memory -> visible to the async proxy (wgmma operand reads)
+__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+// Byte offset of 16-byte chunk `chunk` (0..7) of row `row` in a K-major SWIZZLE_128B tile (rows of 128 B, base 1024-aligned)
+__device__ __forceinline__ uint32_t swz128(int row, int chunk) {
+    return (uint32_t)(row >> 3) * 1024u + (uint32_t)(row & 7) * 128u + (uint32_t)((chunk ^ (row & 7)) << 4);
+}
+// wgmma shared-memory matrix descriptor of a K-major SWIZZLE_128B tile: rows of 128 B, 8-row groups 1024 B apart (stride
+// byte offset); the leading byte offset is unused when K fits one swizzle atom.  A k-block of 16 f16 starts 32 B further.
+__device__ __forceinline__ uint64_t wgmma_desc(uint32_t smem_addr) {
+    return (uint64_t)((smem_addr & 0x3FFFF) >> 4) | ((uint64_t)1 << 16) | ((uint64_t)(1024 >> 4) << 32) | ((uint64_t)1 << 62);
+}
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N_PENDING>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N_PENDING) : "memory"); }
+// D[64 x 16] += A[64 x 16] . B[16 x 16]^T, both operands K-major in shared memory, f16 in, fp32 accumulate
+// accumulate == 0: D = A . B^T (the old contents of d are ignored)
+__device__ __forceinline__ void wgmma_m64n16k16(float (&d)[8], uint64_t da, uint64_t db, int accumulate) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7}, %8, %9, p, 1, 1, 0, 0;\n\t}"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+                 : "l"(da), "l"(db), "r"(accumulate) : "memory");
 }
 
 __global__ void __launch_bounds__(G8_THREADS, 1) gat128_recur_kernel(Gat128Args a) {
     extern __shared__ unsigned char g8_raw[];
-    // warp index through a shuffle: warp-uniform for the compiler, so the MMA operands stay in uniform registers (no per-operand
-    // register-to-uniform waterfall around each of the 72 tcgen05.mma of an item-step)
-    const int tid = threadIdx.x, lane = tid & 31, warp = __shfl_sync(0xffffffffu, tid >> 5, 0);
-    const int grp = warp >> 2, u = tid & 127;                       // hidden unit = TMEM lane
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int wg = warp >> 2, q = lane & 3;
     const int ag = blockIdx.y, dir = blockIdx.z;
     const uint32_t raw_u = smem_u32(g8_raw);
     const uint32_t base = (raw_u + 1023u) & ~1023u;
-    unsigned char* gb = g8_raw + (base - raw_u);
-    const uint32_t bars = base + G8_OFF_BAR;
-    auto d_full = [&](int g) { return bars + 8u * g; };
-    const uint32_t tmem_slot = bars + 32u;
-    if (tid == 0) { mbar_init(d_full(0), 1); mbar_init(d_full(1), 1); mbar_init_fence(); }
-    if (warp == 0) tc5_alloc<512>(tmem_slot);
-    tc5_fence_before();
-    __syncthreads();
-    tc5_fence_after();
-    uint32_t tmem_base;
-    asm volatile("ld.shared.b32 %0, [%1];" : "=r"(tmem_base) : "r"(tmem_slot));
-    const uint32_t tlane = tmem_base + ((uint32_t)((warp & 3) * 32) << 16);
+    float* plx = reinterpret_cast<float*>(g8_raw + (base - raw_u) + G8_OFF_PL);
+    auto wtile = [&](int g, int kh, int hl) { return base + G8_OFF_W + (uint32_t)((((g * 2 + wg) * 2 + kh) * 2 + hl) * G8_WTILE); };
 
-    // ---- W_hh -> tensor memory: M-tile m (gate rows 128 m ..) at columns 128 m: 64 columns of f16 hi pairs, 64 of lo pairs ------
+    // ---- W_hh -> shared memory, gate-activation scale folded in (see gat_common.cuh), f16 hi and lo tiles -----------------
     {
-        const float* whh = a.whh + ((int64_t)(ag * 2 + dir) * G3B) * HB;
-        for (int m = grp; m < 3; m += 2) {                          // group 0: r and n rows, group 1: z rows
-            const float ks = m < 2 ? K_RZ : K_N;                    // gate-activation scale folded in (see gat_common.cuh)
-            const float* wrow = whh + (int64_t)(m * HB + u) * HB;
-#pragma unroll 1
-            for (int kc = 0; kc < 4; ++kc) {                        // 32 k at a time
-                uint32_t hi[16], lo[16];
-#pragma unroll
-                for (int q = 0; q < 8; ++q) {
-                    const float4 w = *reinterpret_cast<const float4*>(wrow + 32 * kc + 4 * q);
-                    split_f16(ks * w.x, ks * w.y, hi[2 * q], lo[2 * q]);
-                    split_f16(ks * w.z, ks * w.w, hi[2 * q + 1], lo[2 * q + 1]);
-                }
-                tc5_st16(tlane + m * 128 + 16 * kc, hi);
-                tc5_st16(tlane + m * 128 + 64 + 16 * kc, lo);
-            }
+        const float* whh = a.whh + (int64_t)(ag * 2 + dir) * G3B * HB;
+        for (int idx = tid; idx < G3B * (HB / 8); idx += G8_THREADS) {
+            const int row = idx >> 4, c16 = idx & 15;                // gate row, chunk of 8 k
+            const int g = row >> 7, w = (row >> 6) & 1, r = row & 63, kh = c16 >> 3;
+            const float ks = g < 2 ? K_RZ : K_N;
+            const float4 x0 = *reinterpret_cast<const float4*>(whh + (int64_t)row * HB + 8 * c16);
+            const float4 x1 = *reinterpret_cast<const float4*>(whh + (int64_t)row * HB + 8 * c16 + 4);
+            uint32_t hi[4], lo[4];
+            split_f16(ks * x0.x, ks * x0.y, hi[0], lo[0]);
+            split_f16(ks * x0.z, ks * x0.w, hi[1], lo[1]);
+            split_f16(ks * x1.x, ks * x1.y, hi[2], lo[2]);
+            split_f16(ks * x1.z, ks * x1.w, hi[3], lo[3]);
+            const uint32_t t = base + G8_OFF_W + (uint32_t)((((g * 2 + w) * 2 + kh) * 2) * G8_WTILE) + swz128(r, c16 & 7);
+            sts128(t, hi[0], hi[1], hi[2], hi[3]);
+            sts128(t + G8_WTILE, lo[0], lo[1], lo[2], lo[3]);
         }
-        asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
     }
-    const float bn = K_N * a.bhn[(ag * 2 + dir) * HB + u];
-    const float lwu = a.lw[(ag * 2 + dir) * HB + u];
-    const uint32_t bt = base + G8_OFF_BT + grp * G8_BT_BYTES;       // this group's h^T operand tile
-    float* qbuf = reinterpret_cast<float*>(gb + G8_OFF_Q + grp * 2 * G8_Q_BYTES);
-    float* plx = reinterpret_cast<float*>(gb + G8_OFF_PL) + grp * (2 * 4 * NB);
-    const uint32_t d_col = G8_D_COL + grp * 48;
-    const bool issuer_warp = (warp & 3) == 0;                       // warp-uniform; one elected lane issues
-    constexpr uint32_t IDESC = tc5_idesc(128, NB);
-    tc5_fence_before();
-    __syncthreads();                                                // W complete in TMEM before any product
-    tc5_fence_after();
+    // this thread's accumulator elements (m64n16 fragment): rows = units u0, u0 + 8; columns = chains 2q, 2q+1 (j = 0) and
+    // 8 + 2q, 9 + 2q (j = 1); element 4 j + 2 rr + e = (unit u0 + 8 rr, chain 8 j + 2 q + e)
+    const int u0 = 64 * wg + 16 * (warp & 3) + (lane >> 2);
+    const int uu[2] = {u0, u0 + 8};
+    float bn[2], lwu[2];
+#pragma unroll
+    for (int rr = 0; rr < 2; ++rr) {
+        bn[rr] = K_N * a.bhn[(ag * 2 + dir) * HB + uu[rr]];
+        lwu[rr] = a.lw[(ag * 2 + dir) * HB + uu[rr]];
+    }
 
     const int64_t it0 = (int64_t)blockIdx.x * a.items_per_cta;
     const int64_t it1 = it0 + a.items_per_cta < a.n_items ? it0 + a.items_per_cta : a.n_items;
     const int64_t pq_stride_dir = (int64_t)a.n_agents * a.n_items * NB * G3B;
     const float* Pd = a.P + dir * pq_stride_dir + (int64_t)ag * a.n_items * NB * G3B;
     const float* Qd = a.Q + dir * pq_stride_dir + (int64_t)ag * a.n_items * NB * G3B;
-    auto load_q = [&](int64_t item, int buf) {                      // one item's Q table: 24 KB, 16-byte cp.async by the group's 128 threads
-        const float* src = Qd + item * NB * G3B;
-        const uint32_t dst = smem_u32(qbuf) + buf * G8_Q_BYTES;
-        for (int c = u; c < G8_Q_BYTES / 16; c += 128) cp_async16(dst + 16 * c, src + 4 * c);
-        asm volatile("cp.async.commit_group;" ::: "memory");
-    };
-    uint32_t phase = 0;
+    const f32x2 one2 = pk2(1.0f, 1.0f), mtwo2 = pk2(-2.0f, -2.0f);
     int buf = 0;
-    if (it0 + grp < it1) load_q(it0 + grp, 0);
-    for (int64_t item = it0 + grp; item < it1; item += 2, buf ^= 1) {
-        // ---- per item: P into registers (pairs over adjacent chains), h = 0, operand tile = 0 ---------------------------
-        f32x2 P2[3][NB / 2];
+    for (int64_t item = it0; item < it1; ++item) {
+        // ---- per item: P into registers, h = 0, operand tile = 0 -----------------------------------------------------------
+        f32x2 P2[3][2][2];                                          // [gate][rr][j]: (chain 8 j + 2 q, +1) of unit uu[rr]
         {
-            const float* pp = Pd + item * NB * G3B + u;
+            const float* pp = Pd + item * NB * G3B;
 #pragma unroll
-            for (int g3 = 0; g3 < 3; ++g3)
+            for (int g = 0; g < 3; ++g)
 #pragma unroll
-                for (int c2 = 0; c2 < NB / 2; ++c2)
-                    P2[g3][c2] = pk2(pp[(2 * c2) * G3B + g3 * HB], pp[(2 * c2 + 1) * G3B + g3 * HB]);
-        }
-        f32x2 h2[NB / 2];
+                for (int rr = 0; rr < 2; ++rr)
 #pragma unroll
-        for (int c2 = 0; c2 < NB / 2; ++c2) h2[c2] = pk2(0.f, 0.f);
-        {
-            const uint32_t z = bt + 64 * u;                         // 8 KB / 128 threads
-#pragma unroll
-            for (int q = 0; q < 4; ++q) asm volatile("st.shared.v4.u32 [%0], {%1,%1,%1,%1};" ::"r"(z + 16 * q), "r"(0u) : "memory");
-        }
-        if (item + 2 < it1) load_q(item + 2, buf ^ 1);               // next item's Q while this one runs
-        if (item + 2 < it1) asm volatile("cp.async.wait_group 1;" ::: "memory");
-        else asm volatile("cp.async.wait_group 0;" ::: "memory");
-        fence_proxy_async();
-        tc5_fence_before();
-        asm volatile("barrier.sync %0, 128;" ::"r"(1 + grp) : "memory");
-        const float* qt = qbuf + buf * (NB * G3B);
-        auto issue = [&]() {                                        // D^T = W_hh h^T for this group's item: 3 M-tiles x 24 MMAs
-            tc5_fence_after();
-#pragma unroll
-            for (int m = 0; m < 3; ++m) {
-                const uint32_t dst = tmem_base + d_col + 16 * m;
-                const uint32_t wa = tmem_base + m * 128;
-#pragma unroll
-                for (int pass = 0; pass < 3; ++pass) {              // hi*hi, lo*hi (h lo x W hi), hi*lo (h hi x W lo)
-                    const uint32_t wofs = pass == 2 ? 64u : 0u;     // W lo columns
-                    const uint32_t hsub = pass == 1 ? 2u : 0u;      // h lo sub-tiles
-#pragma unroll
-                    for (int kb = 0; kb < 8; ++kb) {
-                        const uint64_t db = tc5_smem_desc(bt + (hsub + (kb >> 2)) * (NB * 128)) + 2 * (kb & 3);
-                        tc5_mma_ts(dst, wa + wofs + 8 * kb, db, IDESC, (pass | kb) != 0);
+                    for (int j = 0; j < 2; ++j) {
+                        const int c = 8 * j + 2 * q;
+                        P2[g][rr][j] = pk2(pp[c * G3B + g * HB + uu[rr]], pp[(c + 1) * G3B + g * HB + uu[rr]]);
                     }
-                }
-            }
-            tc5_commit(d_full(grp));
-        };
-        if (issuer_warp) { if (elect_one()) issue(); }              // step 0 (h = 0)
+        }
+        f32x2 h2[2][2];
+#pragma unroll
+        for (int rr = 0; rr < 2; ++rr) h2[rr][0] = h2[rr][1] = pk2(0.f, 0.f);
+        {
+            const uint32_t z = base + G8_OFF_BT + buf * G8_BT_BYTES + 32 * tid;     // 8 KB / 256 threads
+            sts128(z, 0u, 0u, 0u, 0u);
+            sts128(z + 16, 0u, 0u, 0u, 0u);
+        }
+        fence_proxy_async();
+        __syncthreads();
+        const float* qt = Qd + item * NB * G3B;
         for (int step = 0; step < STEPS; ++step) {
             const int s = dir ? STEPS - 1 - step : step;
-            mbar_wait(d_full(grp), phase & 1);
-            ++phase;
-            tc5_fence_after();
-            float dr[NB], dz[NB], dn[NB];
-            tc5_ld16_nowait(tlane + d_col, dr);
-            tc5_ld16_nowait(tlane + d_col + 16, dz);
-            tc5_ld16_nowait(tlane + d_col + 32, dn);
-            // neighbour of ego i at position s: j = s < i ? s : s + 1 -> chains 0..s read Q row s+1, chains s+1.. read row s
-            const float* qa = qt + s * G3B + u;                     // row s
-            const float* qb = qa + G3B;                             // row s + 1
-            const float qr_a = qa[0], qz_a = qa[HB], qn_a = qa[2 * HB];
-            const float qr_b = qb[0], qz_b = qb[HB], qn_b = qb[2 * HB];
-            tc5_wait_ld16x3(dr, dz, dn);
-            const f32x2 one2 = pk2(1.0f, 1.0f), mtwo2 = pk2(-2.0f, -2.0f), bn2 = pk2(bn, bn), lw2 = pk2(lwu, lwu);
-            f32x2 pl2[NB / 2];
-            uint32_t hh[NB / 2], hl[NB / 2];
+            // neighbour of ego c at position s: j = s < c ? s : s + 1 -> chains 0..s read Q row s+1, chains s+1.. read row s.
+            // Issued before the product so that the L2 latency overlaps it.
+            float qa[3][2], qb[3][2];
 #pragma unroll
-            for (int c4 = 0; c4 < NB / 4; ++c4) {                   // four chains at a time (one shared rcp per gate)
-                const int c0 = 4 * c4;
-                auto qsel = [&](float qa_, float qb_, int c) { return s < c ? qa_ : qb_; };
-                const f32x2 qr0 = pk2(qsel(qr_a, qr_b, c0), qsel(qr_a, qr_b, c0 + 1)), qr1 = pk2(qsel(qr_a, qr_b, c0 + 2), qsel(qr_a, qr_b, c0 + 3));
-                const f32x2 qz0 = pk2(qsel(qz_a, qz_b, c0), qsel(qz_a, qz_b, c0 + 1)), qz1 = pk2(qsel(qz_a, qz_b, c0 + 2), qsel(qz_a, qz_b, c0 + 3));
-                const f32x2 qn0 = pk2(qsel(qn_a, qn_b, c0), qsel(qn_a, qn_b, c0 + 1)), qn1 = pk2(qsel(qn_a, qn_b, c0 + 2), qsel(qn_a, qn_b, c0 + 3));
+            for (int g = 0; g < 3; ++g)
+#pragma unroll
+                for (int rr = 0; rr < 2; ++rr) {
+                    qa[g][rr] = qt[s * G3B + g * HB + uu[rr]];
+                    qb[g][rr] = qt[(s + 1) * G3B + g * HB + uu[rr]];
+                }
+            // D^T = W_hh h^T for this warpgroup's 64 units: 3 gates x 3 passes x 8 k-blocks
+            float acc[3][8];
+            const uint32_t bt = base + G8_OFF_BT + buf * G8_BT_BYTES;
+            wgmma_fence();
+#pragma unroll
+            for (int g = 0; g < 3; ++g)
+#pragma unroll
+                for (int pass = 0; pass < 3; ++pass) {              // hi*hi, W hi x h lo, W lo x h hi
+                    const int hl = pass == 2 ? 1 : 0;
+                    const uint32_t hsub = pass == 1 ? 2u : 0u;
+#pragma unroll
+                    for (int kb = 0; kb < 8; ++kb) {
+                        const uint64_t da = wgmma_desc(wtile(g, kb >> 2, hl) + 32u * (kb & 3));
+                        const uint64_t db = wgmma_desc(bt + (hsub + (kb >> 2)) * (NB * 128) + 32u * (kb & 3));
+                        wgmma_m64n16k16(acc[g], da, db, (pass | kb) != 0);
+                    }
+                }
+            wgmma_commit();
+            wgmma_wait<0>();
+            // ---- gates on (chain, chain + 1) pairs; four reciprocals per rcp.approx --------------------------------------------
+            auto qsel = [&](float qa_, float qb_, int c) { return s < c ? qa_ : qb_; };
+#pragma unroll
+            for (int rr = 0; rr < 2; ++rr) {
+                f32x2 d[3][2], qv[3][2];
+#pragma unroll
+                for (int g = 0; g < 3; ++g)
+#pragma unroll
+                    for (int j = 0; j < 2; ++j) {
+                        const int c = 8 * j + 2 * q;
+                        d[g][j] = pk2(acc[g][4 * j + 2 * rr], acc[g][4 * j + 2 * rr + 1]);
+                        qv[g][j] = pk2(qsel(qa[g][rr], qb[g][rr], c), qsel(qa[g][rr], qb[g][rr], c + 1));
+                    }
+                const f32x2 bn2 = pk2(bn[rr], bn[rr]);
                 f32x2 r0, r1, z0, z1, i0, i1;
-                sigmoid4_den(add2(add2(pk2(dr[c0], dr[c0 + 1]), P2[0][2 * c4]), qr0),
-                             add2(add2(pk2(dr[c0 + 2], dr[c0 + 3]), P2[0][2 * c4 + 1]), qr1), r0, r1);
-                sigmoid4_den(add2(add2(pk2(dz[c0], dz[c0 + 1]), P2[1][2 * c4]), qz0),
-                             add2(add2(pk2(dz[c0 + 2], dz[c0 + 3]), P2[1][2 * c4 + 1]), qz1), z0, z1);
-                sigmoid4_den(fma2(r0, add2(pk2(dn[c0], dn[c0 + 1]), bn2), add2(P2[2][2 * c4], qn0)),
-                             fma2(r1, add2(pk2(dn[c0 + 2], dn[c0 + 3]), bn2), add2(P2[2][2 * c4 + 1], qn1)), i0, i1);
+                sigmoid4_den(add2(add2(d[0][0], P2[0][rr][0]), qv[0][0]), add2(add2(d[0][1], P2[0][rr][1]), qv[0][1]), r0, r1);
+                sigmoid4_den(add2(add2(d[1][0], P2[1][rr][0]), qv[1][0]), add2(add2(d[1][1], P2[1][rr][1]), qv[1][1]), z0, z1);
+                sigmoid4_den(fma2(r0, add2(d[2][0], bn2), add2(P2[2][rr][0], qv[2][0])),
+                             fma2(r1, add2(d[2][1], bn2), add2(P2[2][rr][1], qv[2][1])), i0, i1);
                 const f32x2 n0 = fma2(mtwo2, i0, one2), n1 = fma2(mtwo2, i1, one2);
-                h2[2 * c4] = fma2(z0, sub2(h2[2 * c4], n0), n0);
-                h2[2 * c4 + 1] = fma2(z1, sub2(h2[2 * c4 + 1], n1), n1);
-                pl2[2 * c4] = mul2(lw2, h2[2 * c4]);
-                pl2[2 * c4 + 1] = mul2(lw2, h2[2 * c4 + 1]);
-                split_f16p(h2[2 * c4], hh[2 * c4], hl[2 * c4]);     // (chain c0, c0+1) halves of unit u
-                split_f16p(h2[2 * c4 + 1], hh[2 * c4 + 1], hl[2 * c4 + 1]);
+                h2[rr][0] = fma2(z0, sub2(h2[rr][0], n0), n0);
+                h2[rr][1] = fma2(z1, sub2(h2[rr][1], n1), n1);
             }
-            // h^T tile: element (chain c, k = u): sub-tile u >> 6 (hi) / 2 + (u >> 6) (lo), row c, 16-byte chunk (u & 63) >> 3 swizzled
+            // ---- h^T into the other operand tile: element (chain c, k = unit u): sub-tile u >> 6 (hi) / 2 + (u >> 6) (lo) -------
             {
-                const uint32_t sub = bt + (uint32_t)(u >> 6) * (NB * 128), ch = (uint32_t)(u & 63) >> 3, in = (uint32_t)(u & 7) * 2;
+                const uint32_t nt = base + G8_OFF_BT + (buf ^ 1) * G8_BT_BYTES;
 #pragma unroll
-                for (int c2 = 0; c2 < NB / 2; ++c2) {
+                for (int rr = 0; rr < 2; ++rr) {
+                    const int u = uu[rr];
+                    const uint32_t sub = nt + (uint32_t)(u >> 6) * (NB * 128), ch = (uint32_t)(u & 63) >> 3, in = (uint32_t)(u & 7) * 2;
 #pragma unroll
-                    for (int w2 = 0; w2 < 2; ++w2) {
-                        const uint32_t c = 2 * c2 + w2;
-                        const uint32_t off = (c >> 3) * 1024u + (c & 7) * 128u + ((ch ^ (c & 7)) << 4) + in;
-                        sts16(sub + off, (uint16_t)(w2 ? hh[c2] >> 16 : hh[c2] & 0xffffu));
-                        sts16(sub + 2 * (NB * 128) + off, (uint16_t)(w2 ? hl[c2] >> 16 : hl[c2] & 0xffffu));
+                    for (int j = 0; j < 2; ++j) {
+                        uint32_t hh, hl;
+                        split_f16p(h2[rr][j], hh, hl);
+#pragma unroll
+                        for (int e = 0; e < 2; ++e) {
+                            const uint32_t c = 8 * j + 2 * q + e;
+                            const uint32_t off = (c >> 3) * 1024u + (c & 7) * 128u + ((ch ^ (c & 7)) << 4) + in;
+                            sts16(sub + off, (uint16_t)(e ? hh >> 16 : hh & 0xffffu));
+                            sts16(sub + 2 * (NB * 128) + off, (uint16_t)(e ? hl >> 16 : hl & 0xffffu));
+                        }
                     }
                 }
             }
-            // hard-attention logit difference of every chain: sum over the 128 units = warp butterfly, then the 4 warps through shared memory
-            float* plw = plx + (step & 1) * (4 * NB) + (warp & 3) * NB;
+            // ---- hard-attention logit difference of every chain: sum over the 128 units = the 8 fragment rows of a warp, then
+            //      the 8 warps through shared memory
+            {
+                float* plw = plx + (step & 1) * (8 * NB) + warp * NB;
 #pragma unroll
-            for (int c2 = 0; c2 < NB / 2; ++c2) {
-                float pa, pb;
-                upk2(pl2[c2], pa, pb);
+                for (int j = 0; j < 2; ++j) {
+                    float pa, pb, ra, rb;
+                    upk2(h2[0][j], pa, pb);
+                    upk2(h2[1][j], ra, rb);
+                    pa = fmaf(lwu[1], ra, lwu[0] * pa);
+                    pb = fmaf(lwu[1], rb, lwu[0] * pb);
 #pragma unroll
-                for (int o = 16; o > 0; o >>= 1) { pa += __shfl_xor_sync(0xffffffffu, pa, o); pb += __shfl_xor_sync(0xffffffffu, pb, o); }
-                if (lane == 0) { plw[2 * c2] = pa; plw[2 * c2 + 1] = pb; }
+                    for (int o = 4; o < 32; o <<= 1) { pa += __shfl_xor_sync(0xffffffffu, pa, o); pb += __shfl_xor_sync(0xffffffffu, pb, o); }
+                    if (lane < 4) { plw[8 * j + 2 * q] = pa; plw[8 * j + 2 * q + 1] = pb; }
+                }
             }
             fence_proxy_async();
-            tc5_fence_before();
-            asm volatile("barrier.sync %0, 128;" ::"r"(1 + grp) : "memory");
-            if (issuer_warp && step + 1 < STEPS) { if (elect_one()) issue(); }
-            if (u < NB) {                                           // dl[item][dir][s][i]
-                const float* px = plx + (step & 1) * (4 * NB) + u;
-                a.dl[((((int64_t)ag * a.n_items + item) * 2 + dir) * STEPS + s) * NB + u] = ((px[0] + px[NB]) + px[2 * NB]) + px[3 * NB];
+            __syncthreads();
+            buf ^= 1;
+            if (tid < NB) {                                         // dl[item][dir][s][i]
+                const float* px = plx + (step & 1) * (8 * NB) + tid;
+                float v = px[0];
+#pragma unroll
+                for (int w8 = 1; w8 < 8; ++w8) v += px[w8 * NB];
+                a.dl[((((int64_t)ag * a.n_items + item) * 2 + dir) * STEPS + s) * NB + tid] = v;
             }
         }
     }
-    tc5_fence_before();
-    __syncthreads();
-    if (warp == 0) { tc5_fence_after(); tc5_dealloc<512>(tmem_base); }
 }
 
 // ---- attention over one item (16 slots): scores, gumbel hard gate, soft-max, aggregation ---------------------------------
@@ -354,11 +343,11 @@ extern "C" int iplan_gat128_recur(const float* P, const float* Q, const float* w
     }
     Gat128Args a;
     a.P = P; a.Q = Q; a.whh = whh; a.bhn = bhn; a.lw = lw; a.dl = dl; a.n_agents = n_agents; a.n_items = n_items;
-    // (agent-net, direction) pairs x chunks: whole waves of 148 CTAs as nearly as possible, at least 2 items per CTA
+    // (agent-net, direction) pairs x chunks: about eight waves of CTAs, so that the last, partial wave is short; every CTA
+    // stages its W_hh once and then walks its items
     const int pairs = 2 * n_agents;
-    int chunks = (148 * 3 + pairs - 1) / pairs;
-    if ((int64_t)chunks * 2 > n_items) chunks = (int)((n_items + 1) / 2);
-    if (chunks < 1) chunks = 1;
+    int chunks = (sm_count() * 8 + pairs - 1) / pairs;
+    if (chunks > n_items) chunks = (int)n_items;
     a.items_per_cta = (int)((n_items + chunks - 1) / chunks);
     chunks = (int)((n_items + a.items_per_cta - 1) / a.items_per_cta);
     gat128_recur_kernel<<<dim3((unsigned)chunks, (unsigned)n_agents, 2), G8_THREADS, G8_SMEM, (cudaStream_t)stream>>>(a);
@@ -378,7 +367,7 @@ extern "C" int iplan_gat128_attend(const float* qkv, const float* v_bias, const 
 
 extern "C" int iplan_gat128_gates(const float* gi, const float* gh, const float* hprev, float* out, int64_t rows, void* stream) {
     IPLAN_REQUIRE(gi && gh && hprev && out && rows > 0, "gat128_gates: bad arguments");
-    gat128_gates_kernel<<<148 * 8, 256, 0, (cudaStream_t)stream>>>(gi, gh, hprev, out, rows * HB);
+    gat128_gates_kernel<<<sm_count() * 8, 256, 0, (cudaStream_t)stream>>>(gi, gh, hprev, out, rows * HB);
     count_launch();
     return check_launch("gat128_gates");
 }

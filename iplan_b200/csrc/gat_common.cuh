@@ -1,4 +1,4 @@
-// Shared pieces of the K1 kernels (gat_step.cu: mma.sync recurrence + attention; gat_tc5.cu: tcgen05 recurrence):
+// Shared pieces of the GAT kernels (gat_step.cu: K1 recurrence + attention; gat128.cu: the 128-wide recurrence):
 // launch arguments, gate-activation constants, packed-fp32 arithmetic and the f16 hi/lo split.
 #pragma once
 #include <cuda_fp16.h>
@@ -38,19 +38,18 @@ constexpr float K_N = 2.8853900817779268f;        //  2 log2(e)
 __device__ __forceinline__ float ex2_approx(float x) { float y; asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
 __device__ __forceinline__ float rcp_approx(float x) { float y; asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
 
-// Packed fp32 pairs (sm_100a FADD2 / FMUL2 / FFMA2): the gate math of the recurrence is issue-slot
-// bound, and an accumulator fragment is two (col, col+1) pairs, so every elementwise op is done on
-// pairs.  A pair lives in a 64-bit register (lo = first element).
-typedef unsigned long long f32x2;
-__device__ __forceinline__ f32x2 pk2(float a, float b) { f32x2 r; asm("mov.b64 %0, {%1,%2};" : "=l"(r) : "f"(a), "f"(b)); return r; }
-__device__ __forceinline__ void upk2(f32x2 v, float& a, float& b) { asm("mov.b64 {%0,%1}, %2;" : "=f"(a), "=f"(b) : "l"(v)); }
-__device__ __forceinline__ f32x2 add2(f32x2 a, f32x2 b) { f32x2 r; asm("add.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b)); return r; }
-__device__ __forceinline__ f32x2 sub2(f32x2 a, f32x2 b) { f32x2 r; asm("sub.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b)); return r; }
-__device__ __forceinline__ f32x2 mul2(f32x2 a, f32x2 b) { f32x2 r; asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b)); return r; }
-__device__ __forceinline__ f32x2 fma2(f32x2 a, f32x2 b, f32x2 c) { f32x2 r; asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(r) : "l"(a), "l"(b), "l"(c)); return r; }
+// fp32 pairs: an accumulator fragment is two (col, col+1) pairs, so the gate math is written on pairs.
+// sm_90 has no packed fp32 instructions; each pair op is two scalar round-to-nearest ops.
+typedef float2 f32x2;
+__device__ __forceinline__ f32x2 pk2(float a, float b) { return make_float2(a, b); }
+__device__ __forceinline__ void upk2(f32x2 v, float& a, float& b) { a = v.x; b = v.y; }
+__device__ __forceinline__ f32x2 add2(f32x2 a, f32x2 b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
+__device__ __forceinline__ f32x2 sub2(f32x2 a, f32x2 b) { return make_float2(__fsub_rn(a.x, b.x), __fsub_rn(a.y, b.y)); }
+__device__ __forceinline__ f32x2 mul2(f32x2 a, f32x2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
+__device__ __forceinline__ f32x2 fma2(f32x2 a, f32x2 b, f32x2 c) { return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y)); }
 __device__ __forceinline__ f32x2 lds64(const float* p) {
     f32x2 v;
-    asm volatile("ld.shared.b64 %0, [%1];" : "=l"(v) : "r"((uint32_t)__cvta_generic_to_shared(p)));
+    asm volatile("ld.shared.v2.f32 {%0,%1}, [%2];" : "=f"(v.x), "=f"(v.y) : "r"((uint32_t)__cvta_generic_to_shared(p)));
     return v;
 }
 
@@ -95,9 +94,5 @@ __device__ __forceinline__ void split_f16(float x, float y, uint32_t& hi, uint32
     hi = *reinterpret_cast<const uint32_t*>(&h);
     lo = *reinterpret_cast<const uint32_t*>(&l);
 }
-
-// tcgen05 kernel (gat_tc5.cu): fused = the whole step in one launch; else the recurrence only (same dl scratch layout as
-// gat_recur_kernel, consumed by gat_attend_kernel)
-int launch_gat_tc5(const GatArgs& a, int n_agents, bool fused, bool* did_fuse, cudaStream_t st);
 
 }  // namespace iplan

@@ -35,7 +35,6 @@
 // HBM traffic per (b,a): read N*(o+L+32) floats, write N*32 floats; weights (28.8k floats)
 // and the dl scratch come from L2.
 #include <cuda_fp16.h>
-#include <stdlib.h>
 
 #include <type_traits>
 
@@ -402,7 +401,7 @@ __global__ void __launch_bounds__(GAT_THREADS, 2) gat_attend_kernel(GatArgs a) {
     for (int i = warp; i < N; i += GAT_WARPS) {
         float sc[2], hd[2];
         uint4 rnd[2] = {make_uint4(0u, 0u, 0u, 0u), make_uint4(0u, 0u, 0u, 0u)};
-        if (!a.gumbel) {                                                  // Philox key (ego, j >> 2), word j & 3 (as gat_tc5_kernel)
+        if (!a.gumbel) {                                                  // Philox key (ego, j >> 2), word j & 3
 #pragma unroll
             for (int u = 0; u < 2; ++u) {
                 const int64_t key = (((int64_t)ag * a.n_envs + b) * N + i) * 16 + ((lane + 32 * u) >> 2);
@@ -461,26 +460,6 @@ __global__ void __launch_bounds__(GAT_THREADS, 2) gat_attend_kernel(GatArgs a) {
 
 }  // namespace iplan
 
-namespace iplan {
-// 0 = ONE fused tcgen05 kernel (gat_tc5.cu, default), 1 = mma.sync recurrence + attention kernel (the cross-check),
-// 2 = tcgen05 recurrence + attention kernel
-static int g_gat_impl = -1;
-static int gat_impl() {
-    if (g_gat_impl < 0) {
-        const char* e = getenv("IPLAN_GAT_IMPL");
-        g_gat_impl = (e && (e[0] == '1' || e[0] == 'm')) ? 1 : ((e && e[0] == '2') ? 2 : 0);
-    }
-    return g_gat_impl;
-}
-}  // namespace iplan
-
-extern "C" int iplan_gat_set_impl(int impl) {
-    IPLAN_REQUIRE(impl >= 0 && impl <= 2, "gat_set_impl: %d not in {0 (fused tcgen05), 1 (mma.sync + attention), 2 (tcgen05 recurrence + attention)}", impl);
-    iplan::g_gat_impl = impl;
-    return 0;
-}
-extern "C" int iplan_gat_get_impl(void) { return iplan::gat_impl(); }
-
 extern "C" int64_t iplan_gat_scratch_floats(int n_envs, int n_agents, int n_slots) {
     return (int64_t)n_envs * n_agents * 2 * (n_slots - 1) * iplan::DLP;
 }
@@ -519,22 +498,14 @@ extern "C" int iplan_gat_step_ex(const float* gat_params, int64_t param_stride,
         conf_a = smem_a;
     }
     if (ev_begin) cudaEventRecord((cudaEvent_t)ev_begin, (cudaStream_t)stream);
-    int rc;
-    bool fused = false;
-    if (gat_impl() != 1) {
-        rc = launch_gat_tc5(a, n_agents, gat_impl() == 0, &fused, (cudaStream_t)stream);
-    } else {
-        gat_recur_kernel<<<dim3(n_envs, n_agents, 2), REC_THREADS, smem_r, (cudaStream_t)stream>>>(a);
-        count_launch();
-        rc = check_launch("gat_step(recur)");
-    }
+    gat_recur_kernel<<<dim3(n_envs, n_agents, 2), REC_THREADS, smem_r, (cudaStream_t)stream>>>(a);
+    count_launch();
+    int rc = check_launch("gat_step(recur)");
     if (rc) return rc;
     if (ev_mid) cudaEventRecord((cudaEvent_t)ev_mid, (cudaStream_t)stream);
-    if (!fused) {
-        gat_attend_kernel<<<dim3(n_envs, n_agents), GAT_THREADS, smem_a, (cudaStream_t)stream>>>(a);
-        count_launch();
-        rc = check_launch("gat_step(attend)");
-    }
+    gat_attend_kernel<<<dim3(n_envs, n_agents), GAT_THREADS, smem_a, (cudaStream_t)stream>>>(a);
+    count_launch();
+    rc = check_launch("gat_step(attend)");
     if (ev_end) cudaEventRecord((cudaEvent_t)ev_end, (cudaStream_t)stream);
     return rc;
 }

@@ -618,7 +618,7 @@ using namespace iplan;
 extern "C" int iplan_learner_row_stats(const float* X, int64_t x_stride_agent, int ldx, int feat_dim, int64_t rows,
                                        int n_agents, float* stat, void* stream) {
     IPLAN_REQUIRE(X && stat && rows > 0 && n_agents > 0 && feat_dim > 0 && ldx >= feat_dim, "row_stats: bad arguments");
-    dim3 grid((unsigned)std::min<int64_t>((rows + 7) / 8, 148 * 16), n_agents);
+    dim3 grid((unsigned)std::min<int64_t>((rows + 7) / 8, sm_count() * 16), n_agents);
     row_stats_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(X, x_stride_agent, ldx, feat_dim, rows, stat);
     count_launch();
     return check_launch("row_stats");
@@ -639,7 +639,7 @@ extern "C" int iplan_learner_tail(const iplan_learner_ctx* c, int train, void* s
     RowBuf a1{c->A1, 2 * rows * RH, rows * RH, RH}, z2{c->Z2, 2 * rows * RH, rows * RH, RH}, a2{c->A2, 2 * rows * RH, rows * RH, RH};
     RowBuf gi{c->GI, 2 * rows * RH3, rows * RH3, RH3}, gh{c->GH, 2 * rows * RH3, rows * RH3, RH3};
     // the stored hidden inputs: type 0 reads rnn_a, type 1 reads rnn_c -> two launches for GH
-    const unsigned rw = (unsigned)std::min<int64_t>((rows + 7) / 8, 148 * 8);
+    const unsigned rw = (unsigned)std::min<int64_t>((rows + 7) / 8, sm_count() * 8);
     const unsigned mt = (unsigned)((rows + 63) / 64), mt128 = (unsigned)((rows + 127) / 128);
     static bool lin_configured = false;
     if (!lin_configured) {
@@ -677,7 +677,10 @@ extern "C" int iplan_learner_tail(const iplan_learner_ctx* c, int train, void* s
         fa.h = h; fa.z1 = z1; fa.a1 = a1; fa.z2 = z2; fa.a2 = a2; fa.stat = c->stat; fa.SM = c->SM; fa.rows = rows;
         const int64_t n_tiles16 = (rows + 15) / 16;
         // one CTA per SM: ctas x (2A nets) CTAs, actor and critic tiles side by side
-        const int ctas = (int)std::min<int64_t>((n_tiles16 + TF_WARPS - 1) / TF_WARPS, std::max(1, 148 / (2 * A)));
+        const int ctas = (int)std::min<int64_t>((n_tiles16 + TF_WARPS - 1) / TF_WARPS, std::max(1, sm_count() / (2 * A)));
+        const DetScratch ds = det_scratch((size_t)2 * A * ctas * TF_WARPS * TF_REC, (size_t)2 * A);
+        if (!ds.part) return -1;                                      // det_scratch set the error text
+        fa.part = ds.part; fa.count = ds.count;
         if (c->n_actions <= 5) tail_fused_kernel<5><<<dim3((unsigned)ctas, 2 * A), TF_THREADS, TF_SMEM, st>>>(fa);
         else tail_fused_kernel<TF_NOUT><<<dim3((unsigned)ctas, 2 * A), TF_THREADS, TF_SMEM, st>>>(fa);
         launches = 1;
@@ -685,17 +688,17 @@ extern "C" int iplan_learner_tail(const iplan_learner_ctx* c, int train, void* s
         const unsigned dw_ctas = (unsigned)std::min<int64_t>(n_tiles64, 32);
         const int dw_tiles = (int)((n_tiles64 + dw_ctas - 1) / dw_ctas);
         // weight gradients (K = rows) + the bias gradients = column sums of the same dY arrays
-        lin64_dw_kernel<192><<<dim3(dw_ctas, 2 * A), 256, Lin64Dw<192>::SMEM, st>>>(gi, a2, G, L.wih, rows, dw_tiles, 2, L.bih); ++launches;
+        if (int rc = launch_lin64_dw<192>(dim3(dw_ctas, 2 * A), st, gi, a2, G, L.wih, rows, dw_tiles, 2, L.bih)) return rc; ++launches;
         {
             RowBuf h0a{const_cast<float*>(c->rnn_a), c->rnn_stride_agent, 0, c->rnn_ld};
             RowBuf h0c{const_cast<float*>(c->rnn_c), c->rnn_stride_agent, 0, c->rnn_ld};
             RowBuf gha{c->GH, 2 * rows * RH3, 0, RH3}, ghc{c->GH + rows * RH3, 2 * rows * RH3, 0, RH3};
             NetGrads Ga{c->g_actor, c->g_actor, c->actor_stride, c->actor_stride};
             NetGrads Gc{c->g_critic, c->g_critic, c->critic_stride, c->critic_stride};
-            lin64_dw_kernel<192><<<dim3(dw_ctas, A), 256, Lin64Dw<192>::SMEM, st>>>(gha, h0a, Ga, L.whh, rows, dw_tiles, 1, L.bhh); ++launches;
-            lin64_dw_kernel<192><<<dim3(dw_ctas, A), 256, Lin64Dw<192>::SMEM, st>>>(ghc, h0c, Gc, L.whh, rows, dw_tiles, 1, L.bhh); ++launches;
+            if (int rc = launch_lin64_dw<192>(dim3(dw_ctas, A), st, gha, h0a, Ga, L.whh, rows, dw_tiles, 1, L.bhh)) return rc; ++launches;
+            if (int rc = launch_lin64_dw<192>(dim3(dw_ctas, A), st, ghc, h0c, Gc, L.whh, rows, dw_tiles, 1, L.bhh)) return rc; ++launches;
         }
-        lin64_dw_kernel<64><<<dim3(dw_ctas, 2 * A), 256, Lin64Dw<64>::SMEM, st>>>(z2, a1, G, L.fc2_w, rows, dw_tiles, 2, L.fc2_b); ++launches;
+        if (int rc = launch_lin64_dw<64>(dim3(dw_ctas, 2 * A), st, z2, a1, G, L.fc2_w, rows, dw_tiles, 2, L.fc2_b)) return rc; ++launches;
         tail_beta_kernel<<<2 * A, RH, 0, st>>>(P, G, c->feat_dim, c->n_actions); ++launches;
         count_launch(launches);
         return check_launch("learner_tail(fused)");
@@ -714,7 +717,7 @@ extern "C" int iplan_learner_tail(const iplan_learner_ctx* c, int train, void* s
         lin64_rows_kernel<64, 192, 128, false><<<dim3(mt128, A), 256, Lin64Rows<64, 192, 128, false>::SMEM, st>>>(h0c, ghc, Pc, L.whh, L.bhh, rows, 1); ++launches;
     }
     {
-        const dim3 hgrid((unsigned)std::min<int64_t>((rows + 7) / 8, 148 * 6), A);
+        const dim3 hgrid((unsigned)std::min<int64_t>((rows + 7) / 8, sm_count() * 6), A);
         if (c->n_actions <= 5) gru_head_kernel<0, 5><<<hgrid, HEAD_THREADS, 0, st>>>(h);
         else gru_head_kernel<0, IPLAN_MAX_ACT><<<hgrid, HEAD_THREADS, 0, st>>>(h);
         gru_head_kernel<1, 1><<<hgrid, HEAD_THREADS, 0, st>>>(h);
@@ -725,19 +728,19 @@ extern "C" int iplan_learner_tail(const iplan_learner_ctx* c, int train, void* s
         const unsigned dw_ctas = (unsigned)std::min<int64_t>(n_tiles64, 32);
         const int dw_tiles = (int)((n_tiles64 + dw_ctas - 1) / dw_ctas);
         // GRU projections: dW_ih = dGI^T A2, dW_hh = dGH^T H0, dA2 = dGI W_ih (into the A2 buffer)
-        lin64_dw_kernel<192><<<dim3(dw_ctas, 2 * A), 256, Lin64Dw<192>::SMEM, st>>>(gi, a2, G, L.wih, rows, dw_tiles, 2); ++launches;
+        if (int rc = launch_lin64_dw<192>(dim3(dw_ctas, 2 * A), st, gi, a2, G, L.wih, rows, dw_tiles, 2)) return rc; ++launches;
         {
             RowBuf h0a{const_cast<float*>(c->rnn_a), c->rnn_stride_agent, 0, c->rnn_ld};
             RowBuf h0c{const_cast<float*>(c->rnn_c), c->rnn_stride_agent, 0, c->rnn_ld};
             RowBuf gha{c->GH, 2 * rows * RH3, 0, RH3}, ghc{c->GH + rows * RH3, 2 * rows * RH3, 0, RH3};
             NetGrads Ga{c->g_actor, c->g_actor, c->actor_stride, c->actor_stride};
             NetGrads Gc{c->g_critic, c->g_critic, c->critic_stride, c->critic_stride};
-            lin64_dw_kernel<192><<<dim3(dw_ctas, A), 256, Lin64Dw<192>::SMEM, st>>>(gha, h0a, Ga, L.whh, rows, dw_tiles, 1); ++launches;
-            lin64_dw_kernel<192><<<dim3(dw_ctas, A), 256, Lin64Dw<192>::SMEM, st>>>(ghc, h0c, Gc, L.whh, rows, dw_tiles, 1); ++launches;
+            if (int rc = launch_lin64_dw<192>(dim3(dw_ctas, A), st, gha, h0a, Ga, L.whh, rows, dw_tiles, 1)) return rc; ++launches;
+            if (int rc = launch_lin64_dw<192>(dim3(dw_ctas, A), st, ghc, h0c, Gc, L.whh, rows, dw_tiles, 1)) return rc; ++launches;
         }
         lin64_rows_kernel<192, 64, 64, true><<<dim3(mt, 2 * A), 128, Lin64Rows<192, 64, 64, true>::SMEM, st>>>(gi, a2, P, L.wih, -1, rows, 2); ++launches;
         ln_relu_bwd_kernel<<<dim3(rw, 2 * A), 256, 0, st>>>(z2, a2, P, G, L.ln2_w, L.ln2_b, L.fc2_b, rows, 2, nullptr, nullptr); ++launches;
-        lin64_dw_kernel<64><<<dim3(dw_ctas, 2 * A), 256, Lin64Dw<64>::SMEM, st>>>(z2, a1, G, L.fc2_w, rows, dw_tiles, 2); ++launches;
+        if (int rc = launch_lin64_dw<64>(dim3(dw_ctas, 2 * A), st, z2, a1, G, L.fc2_w, rows, dw_tiles, 2)) return rc; ++launches;
         lin64_rows_kernel<64, 64, 128, true><<<dim3(mt128, 2 * A), 256, Lin64Rows<64, 64, 128, true>::SMEM, st>>>(z2, a1, P, L.fc2_w, -1, rows, 2); ++launches;
         ln_relu_bwd_kernel<<<dim3(rw, 2 * A), 256, 0, st>>>(z1, a1, P, G, L.ln1_w, L.ln1_b, L.fc1_b, rows, 2, c->stat, c->SM); ++launches;
     }
@@ -783,7 +786,7 @@ extern "C" int iplan_learner_adam(float* params, const float* grads, float* exp_
     cudaError_t e = cudaMemsetAsync(sqnorm_scratch, 0, sizeof(float) * n_agents, st);
     if (e != cudaSuccess) { set_error("adam: memset: %s", cudaGetErrorString(e)); return (int)e; }
     const float inv = 1.0f / grad_scale;
-    grad_sqnorm_kernel<<<dim3(64, n_agents), 256, 0, st>>>(grads, stride, total, inv, sqnorm_scratch);
+    grad_sqnorm_kernel<<<dim3(1, n_agents), 1024, 0, st>>>(grads, stride, total, inv, sqnorm_scratch);   // one block per agent: a fixed summation order
     const double bc1 = 1.0 - pow((double)beta1, step), bc2 = 1.0 - pow((double)beta2, step);
     adam_kernel<<<dim3(128, n_agents), 256, 0, st>>>(params, grads, exp_avg, exp_avg_sq, mask, sqnorm_scratch, stride, total,
                                                      lr, beta1, beta2, eps, (float)bc1, (float)sqrt(bc2), max_norm, inv, stats, stat_col);

@@ -131,10 +131,12 @@ struct Lin64Dw {
     static constexpr int MTW = NO / 64;                  // m-tiles per warp (warp grid 4 x 2)
 };
 
-// bias_off >= 0: also adds the column sums of dY (the gradient of the layer's bias) to Gr[bias_off + n]
+// bias_off >= 0: also adds the column sums of dY (the gradient of the layer's bias) to Gr[bias_off + n].
+// The CTAs of one net (blockIdx.y) store their partial sums in part[blockIdx.y][blockIdx.x][NO * 64 + NO]; the last of them to
+// finish adds those in CTA order (det_last_arrival, count[blockIdx.y]).
 template <int NO>
 __global__ void __launch_bounds__(256) lin64_dw_kernel(RowBuf dy, RowBuf x, NetGrads Gr, int64_t w_off, int64_t rows,
-                                                        int tiles_per_cta, int n_types, int64_t bias_off = -1) {
+                                                        int tiles_per_cta, int n_types, int64_t bias_off, float* part, unsigned* count) {
     using C = Lin64Dw<NO>;
     extern __shared__ __align__(16) unsigned char l64_smem[];
     float* Ds = reinterpret_cast<float*>(l64_smem);       // [64][DP]  dY tile
@@ -215,8 +217,9 @@ __global__ void __launch_bounds__(256) lin64_dw_kernel(RowBuf dy, RowBuf x, NetG
             }
         __syncthreads();
     }
-    if (bias_off >= 0 && tid < NO) atomicAdd(&Gr.net(a, type)[bias_off + tid], colsum);
-    float* gw = Gr.net(a, type) + w_off;
+    constexpr int V = NO * 64 + NO;
+    float* slot = part + ((int64_t)blockIdx.y * gridDim.x + blockIdx.x) * V;
+    if (tid < NO) slot[NO * 64 + tid] = colsum;
 #pragma unroll
     for (int i = 0; i < C::MTW; ++i)
 #pragma unroll
@@ -225,6 +228,26 @@ __global__ void __launch_bounds__(256) lin64_dw_kernel(RowBuf dy, RowBuf x, NetG
             for (int e = 0; e < 4; ++e) {
                 const int m = wm * (NO / 4) + 16 * i + g + ((e & 2) ? 8 : 0);
                 const int n = wn * 32 + 8 * j + 2 * t + (e & 1);
-                atomicAdd(&gw[m * 64 + n], acc[i][j][e]);
+                slot[m * 64 + n] = acc[i][j][e];
             }
+    if (!det_last_arrival(count + blockIdx.y, gridDim.x)) return;
+    const float* slots = part + (int64_t)blockIdx.y * gridDim.x * V;
+    float* gw = Gr.net(a, type) + w_off;
+    for (int idx = tid; idx < V; idx += C::THREADS) {
+        if (idx >= NO * 64 && bias_off < 0) break;
+        float s = 0.0f;
+        for (unsigned c = 0; c < gridDim.x; ++c) s += __ldcg(slots + (int64_t)c * V + idx);
+        if (idx < NO * 64) gw[idx] += s;
+        else Gr.net(a, type)[bias_off + idx - NO * 64] += s;
+    }
+}
+
+// launch with the scratch of the ordered reduction
+template <int NO>
+int launch_lin64_dw(dim3 grid, cudaStream_t st, RowBuf dy, RowBuf x, NetGrads Gr, int64_t w_off, int64_t rows, int tiles_per_cta,
+                    int n_types, int64_t bias_off = -1) {
+    const DetScratch ds = det_scratch((size_t)grid.x * grid.y * (NO * 64 + NO), grid.y);
+    if (!ds.part) return -1;                                      // det_scratch set the error text
+    lin64_dw_kernel<NO><<<grid, 256, Lin64Dw<NO>::SMEM, st>>>(dy, x, Gr, w_off, rows, tiles_per_cta, n_types, bias_off, ds.part, ds.count);
+    return 0;
 }

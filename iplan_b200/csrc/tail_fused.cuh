@@ -53,6 +53,8 @@ struct TfAcc {
     float s[3 + TF_NOUT][32];      // per-lane running sums of row scalars: loss | entropy | ratio | d head_b[l]
 };
 constexpr size_t TF_SMEM = sizeof(TfFrag) + sizeof(TfVec) + TF_WARPS_C * sizeof(TfAcc);
+// one warp's flushed sums: the slot vectors, then the row scalars; a multiple of 4 floats keeps every record 16-byte aligned
+constexpr int TF_REC = (TF_SLOTS * 64 + 3 + TF_NOUT + 3) & ~3;
 
 struct TfArgs {
     HeadArgs h;                    // parameters, targets, loss constants (h.gi / h.gh = the dGI / dGH buffers)
@@ -60,6 +62,8 @@ struct TfArgs {
     const float* stat;             // [A][rows][2] mean / rstd of the input LayerNorm
     float* SM;                     // [A][2][128]  S = colsum(dZ1), M = sum_r dZ1 rstd_r mu_r
     int64_t rows;
+    float* part;                   // [2A][CTAs][TF_WARPS][TF_REC] the warps' sums, reduced in warp order (det_last_arrival)
+    unsigned* count;               // [2A]
 };
 
 // gates with ex2.approx / rcp.approx (abs error ~1e-7, as in K1): sigmoid(x) = 1 / (1 + 2^(-x log2 e)), tanh(x) = 1 - 2 / (1 + 2^(2 x log2 e))
@@ -181,7 +185,7 @@ __device__ __forceinline__ void tf_ln_relu_bwd(const float (&z)[8][4], const flo
 }
 
 // blockIdx.y = 2 * agent + net type (0 actor: NOUT >= n_actions head rows; 1 critic: one head row): actor and critic tiles
-// run side by side so that one launch covers all 148 SMs.  ONE body for both (only the loss section branches on the type):
+// run side by side so that one launch covers all SMs.  ONE body for both (only the loss section branches on the type):
 // two instantiations of this much straight-line code would not stay in the instruction cache.
 template <int NOUT>
 __global__ void __launch_bounds__(TF_THREADS, 1) tail_fused_kernel(TfArgs A) {
@@ -637,30 +641,41 @@ __global__ void __launch_bounds__(TF_THREADS, 1) tail_fused_kernel(TfArgs A) {
             tf_red16(ACC.v[TF_SLOT_M], lane, mv);
         }
     }
-    // ---- the warp's accumulated small gradients -> global memory -----------------------------------------------------------
+    // ---- the warp's accumulated small gradients -> its record; the net's last CTA adds the records in warp order -------------
     __syncwarp();
-    auto flush = [&](int slot, float* dst, float* dst2) {
-        const float2 c = reinterpret_cast<const float2*>(ACC.v[slot])[lane];
-        atomicAdd(dst + 2 * lane, c.x);
-        atomicAdd(dst + 2 * lane + 1, c.y);
-        if (dst2) { atomicAdd(dst2 + 2 * lane, c.x); atomicAdd(dst2 + 2 * lane + 1, c.y); }
-    };
-    flush(TF_SLOT_LN1, gg + L.ln1_w, nullptr);
-    flush(TF_SLOT_LN2, gg + L.ln2_w, nullptr);
-    flush(TF_SLOT_LN3, gg + L.ln3_w, nullptr);
-    flush(TF_SLOT_S, gg + L.fc1_b, smS);                                    // S = colsum(dZ1) is also the fc1 bias gradient
-    flush(TF_SLOT_M, smM, nullptr);
-    for (int l = 0; l < n_out; ++l) flush(TF_SLOT_HEAD + l, gg + L.head_w + l * RH, nullptr);
-    auto flush_scalar = [&](int k, float* dst) {
+    const int64_t n_rec = (int64_t)gridDim.x * TF_WARPS;
+    float* rec = A.part + ((int64_t)blockIdx.y * n_rec + (int64_t)blockIdx.x * TF_WARPS + warp) * TF_REC;
+    for (int sl = 0; sl < TF_SLOTS; ++sl)
+        *reinterpret_cast<float2*>(rec + 64 * sl + 2 * lane) = reinterpret_cast<const float2*>(ACC.v[sl])[lane];
+    for (int k = 0; k < 3 + TF_NOUT; ++k) {
         float v = t == 0 ? ACC.s[k][lane] : 0.0f;                           // one lane per quad: the four hold the same sums
         v += __shfl_xor_sync(0xffffffffu, v, 4);
         v += __shfl_xor_sync(0xffffffffu, v, 8);
         v += __shfl_xor_sync(0xffffffffu, v, 16);
-        if (lane == 0) atomicAdd(dst, v);
-    };
-    flush_scalar(0, &h.stats[a * 8 + (type == 0 ? 0 : 1)]);
-    if (type == 0) { flush_scalar(1, &h.stats[a * 8 + 2]); flush_scalar(2, &h.stats[a * 8 + 3]); }
-    for (int l = 0; l < n_out; ++l) flush_scalar(3 + l, &gg[L.head_b + l]);
+        if (lane == 0) rec[TF_SLOTS * 64 + k] = v;
+    }
+    if (!det_last_arrival(A.count + blockIdx.y, gridDim.x)) return;
+    const float* recs = A.part + (int64_t)blockIdx.y * n_rec * TF_REC;
+    for (int idx = threadIdx.x; idx < TF_REC; idx += TF_THREADS) {
+        float* dst;
+        float* dst2 = nullptr;
+        if (idx < TF_SLOTS * 64) {
+            const int sl = idx >> 6, c = idx & 63;
+            if (sl >= TF_SLOT_HEAD + n_out) continue;
+            dst = sl == TF_SLOT_LN1 ? gg + L.ln1_w + c : sl == TF_SLOT_LN2 ? gg + L.ln2_w + c : sl == TF_SLOT_LN3 ? gg + L.ln3_w + c
+                : sl == TF_SLOT_S ? gg + L.fc1_b + c : sl == TF_SLOT_M ? smM + c : gg + L.head_w + (sl - TF_SLOT_HEAD) * RH + c;
+            if (sl == TF_SLOT_S) dst2 = smS + c;                            // S = colsum(dZ1) is also the fc1 bias gradient
+        } else {
+            const int k = idx - TF_SLOTS * 64;                              // loss | entropy | ratio | d head_b[l]
+            if (k == 0) dst = &h.stats[a * 8 + (type == 0 ? 0 : 1)];
+            else if (k < 3) { if (type != 0) continue; dst = &h.stats[a * 8 + 1 + k]; }
+            else { if (k - 3 >= n_out) continue; dst = &gg[L.head_b + k - 3]; }
+        }
+        float v = 0.0f;
+        for (int64_t r = 0; r < n_rec; ++r) v += __ldcg(recs + r * TF_REC + idx);
+        *dst += v;
+        if (dst2) *dst2 += v;
+    }
 }
 
 // LayerNorm beta gradients and the rest of the gate-bias bookkeeping, from the column sums the weight-gradient kernels

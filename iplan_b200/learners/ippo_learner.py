@@ -243,7 +243,7 @@ class IPPOLearner:
     def _forward(self, w, ctx, X, A, rows, Fp, F, actor, critic, train):
         lib, st = _lib.lib, _lib.stream()
         self._mark("fc1_fwd")
-        _lib.check(lib.iplan_learner_fc1_forward_tc5(      # tcgen05 / TMEM / TMA product (csrc/fc1_tc5.cu)
+        _lib.check(lib.iplan_learner_fc1_forward(
             _lib.ptr(actor), self.stacks["actor"].stride(), _lib.ptr(critic), self.stacks["critic"].stride(),
             _lib.ptr(w["Xh"]), _lib.ptr(w["Xl"]), w["Xh"].stride(0), Fp, F, rows, A, _lib.ptr(w["stat"]),
             _lib.ptr(w["Wh"]), _lib.ptr(w["Wl"]), _lib.ptr(w["ws"]), _lib.ptr(w["cc"]), _lib.ptr(w["Z1"]), st), "fc1_forward")
@@ -311,7 +311,7 @@ class IPPOLearner:
             ga.zero_(); gc.zero_(); w["SM"].zero_()
             self._forward(w, ctx, X, A, rows, Fp, F, actor, critic, train=True)
             self._mark("fc1_bwd")
-            _lib.check(lib.iplan_learner_fc1_backward_tc5(     # tcgen05 / TMEM / TMA product (csrc/fc1_tc5.cu)
+            _lib.check(lib.iplan_learner_fc1_backward(
                 _lib.ptr(actor), self.stacks["actor"].stride(), _lib.ptr(critic), self.stacks["critic"].stride(),
                 _lib.ptr(ga), _lib.ptr(gc), _lib.ptr(w["Xh"]), _lib.ptr(w["Xl"]), w["Xh"].stride(0), Fp, F, rows, A,
                 _lib.ptr(w["Z1"]), _lib.ptr(w["Dh"]), _lib.ptr(w["Dl"]), _lib.ptr(w["gscale"]),
@@ -404,7 +404,7 @@ def eval_rows(mac, agent_id, obs, rnn_states, net, action=None, avail=None):
     lib, st, P = _lib.lib, _lib.stream(), _lib.ptr
     _lib.check(lib.iplan_learner_row_stats(P(X), X.stride(0), Fp, F, rows, 1, P(w["stat"]), st), "row_stats")
     _lib.check(lib.iplan_learner_x_split(P(X), X.numel(), P(w["Xh"]), P(w["Xl"]), st), "x_split")
-    _lib.check(lib.iplan_learner_fc1_forward_tc5(P(actor), mac.actor_stack.stride(), P(critic), mac.critic_stack.stride(),
+    _lib.check(lib.iplan_learner_fc1_forward(P(actor), mac.actor_stack.stride(), P(critic), mac.critic_stack.stride(),
                                              P(w["Xh"]), P(w["Xl"]), w["Xh"].stride(0), Fp, F, rows, 1, P(w["stat"]),
                                              P(w["Wh"]), P(w["Wl"]), P(w["ws"]), P(w["cc"]), P(w["Z1"]), st), "fc1_forward")
     c = _lib.LearnerCtx()

@@ -1,14 +1,14 @@
 """GAT_Net.forward at GAT_hidden_dim = attention_dim = 128 — BASELINE.json configs[4], the synthetic GAT + GRU
 microbench (8192 envs x 32 agent-nets x 16 slots x 128-d features).  The op is the reference's
-``GAT_Net.forward`` (/root/reference/nova/GAT_Net.py:41-142) with ``input_shape = GAT_hidden_dim = attention_dim = 128``
+``GAT_Net.forward`` (nova/GAT_Net.py:41-142) with ``input_shape = GAT_hidden_dim = attention_dim = 128``
 and ``max_vehicle_num = 16``; an "item" is one (env, agent-net) pair = 16 slots.
 
 Split of the work (csrc/gat128.cu has the reasons):
   * the row x weight products over all slots — encode (:50), the factored input projections of the hard-attention GRU
     (W_ih [enc_i ; enc_j] = P_i + Q_j), q | k | v (:99-103), the GRUCell projections (:140) — are plain GEMMs and run
     through the library (cuBLAS fp32 via ``torch.bmm`` / ``torch.baddbmm``, TF32 off);
-  * the bidirectional 15-step recurrence (:57-97), 80 % of the FLOPs, is ``iplan_gat128_recur`` (tcgen05.mma with W_hh
-    resident in tensor memory); attention and the GRUCell gates are ``iplan_gat128_attend`` / ``iplan_gat128_gates``.
+  * the bidirectional 15-step recurrence (:57-97), 80 % of the FLOPs, is ``iplan_gat128_recur`` (wgmma with W_hh
+    resident in shared memory); attention and the GRUCell gates are ``iplan_gat128_attend`` / ``iplan_gat128_gates``.
 
 Parameters use the reference's state_dict key names per agent-net (``load_state_dict(i, sd)`` accepts a reference
 ``GAT_Net(128, args)`` checkpoint).

@@ -155,7 +155,7 @@ class Prediction_policy:
             need = _lib.lib.iplan_gat_scratch_floats(B, A, N)
             if self._scratch is None or self._scratch.numel() < need or self._scratch.device != out.device:
                 self._scratch = torch.empty(need, device=dev, dtype=torch.float32)
-            ends = _lib.wave_chunks(B, lambda e: ((e + 1) // 2) * A)      # K1: one CTA per (2 envs, agent-net)
+            ends = _lib.wave_chunks(B, lambda e: (2 * e * A + 3) // 4)    # K1 recurrence: 2 CTAs per (env, agent-net), 4 resident per SM
             n_chunks = len(ends)
             _lib.check(_lib.lib.iplan_gat_latent_update_host(
                 _lib.ptr(self.stack.flat), self.stack.stride(),

@@ -13,6 +13,7 @@ saves inputs, weights, explicit noise and outputs.  The fixtures pin the oracle
 Nothing on the GPU box reads /root/reference; only the committed *.pt files travel.
 """
 import copy
+import json
 import os
 import sys
 import warnings
@@ -30,6 +31,7 @@ sys.path.insert(1, REPO)
 warnings.filterwarnings("ignore")
 
 from iplan_b200.config import make_args, merged_config  # noqa: E402
+from obs_episode import f32_digest, obs_episode_inputs  # noqa: E402
 
 
 # ---------------------------------------------------------------------------------
@@ -508,6 +510,32 @@ def golden_obs_wrapper():
     print("obs_wrapper: slots used", max(len(x) for r in ids for x in r))
 
 
+def golden_obs_wrapper_episode():
+    """The reference wrapper over a whole 91-observation episode (more observations than the deque's maxlen): digests of
+    every timestep's obs_single_history_output / obs_history_output, of the final obs_history_episode_output(mask), and
+    the slot tables.  Inputs from obs_episode_inputs(np.random.default_rng(99), ...)."""
+    from observation_wrapper import observersation_state_history_wrapper as RefWrapper
+    B, M = 4, 15
+    args = ref_args("highway", batch_size_run=B)
+    A, N, W, o, L = args.n_agents, args.max_vehicle_num, args.max_history_len, args.obs_shape_single, args.episode_limit
+    wr = RefWrapper(args, A, N, L, W)
+    steps, mask = obs_episode_inputs(np.random.default_rng(99), B, A, N, M, o, L)
+    rec = dict(dims=dict(B=B, A=A, N=N, W=W, o=o, M=M, L=L), obs=[], single=[], window=[])
+    for t, obs in enumerate(steps):
+        if t == 0:
+            wr.agent_obs_profile_init(obs)
+        wr.obs_history_create(obs)
+        rec["obs"].append(f32_digest(obs))
+        rec["single"].append(f32_digest(wr.obs_single_history_output()))
+        rec["window"].append(f32_digest(wr.obs_history_output()))
+    rec["ids"] = [[list(map(int, wr.obs_vehicle_id[k][i])) for i in range(A)] for k in range(B)]
+    raw, ep = wr.obs_history_episode_output(mask)
+    rec["raw"], rec["ep"] = f32_digest(raw), f32_digest(ep)
+    with open(os.path.join(HERE, "obs_wrapper_episode.json"), "w") as f:
+        json.dump(rec, f, indent=0)
+    print("obs_wrapper_episode:", len(steps), "steps")
+
+
 if __name__ == "__main__":
     torch.set_num_threads(8)
     golden_config()
@@ -517,6 +545,7 @@ if __name__ == "__main__":
     golden_prediction_learn()
     golden_behavior_learn()
     golden_obs_wrapper()
+    golden_obs_wrapper_episode()
     for f in sorted(os.listdir(HERE)):
         if f.endswith(".pt"):
             print(f, os.path.getsize(os.path.join(HERE, f)) // 1024, "KiB")

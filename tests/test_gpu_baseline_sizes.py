@@ -216,13 +216,13 @@ def test_learner_vs_oracle_baseline_shape():
     assert n_off <= 0.005 * n_all
 
 
-def test_fc1_tcgen05_at_bench_shape():
-    """tools/check_fc1_tc5.py at the benchmark's shape (5 agents x 46 592 rows = 512 envs x 91 x 2 496 features): the tcgen05
-    forward / backward against the mma.sync kernels and an fp64 reference on sampled rows."""
+def test_fc1_at_bench_shape():
+    """tools/check_fc1.py at the benchmark's shape (5 agents x 46 592 rows = 512 envs x 91 x 2 496 features): the fc1
+    forward / backward against an fp64 reference."""
     if not torch.cuda.is_available():
         pytest.skip("needs a CUDA device")
     import importlib.util
-    spec = importlib.util.spec_from_file_location("check_fc1_tc5", os.path.join(ROOT, "tools", "check_fc1_tc5.py"))
+    spec = importlib.util.spec_from_file_location("check_fc1", os.path.join(ROOT, "tools", "check_fc1.py"))
     mod = importlib.util.module_from_spec(spec)
     spec.loader.exec_module(mod)
     assert mod.run(5, 46592, 2485, reps=1) < 1e-5

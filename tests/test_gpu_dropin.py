@@ -82,7 +82,7 @@ def test_reference_runner_body_drives_iplan_b200_objects(own_wrapper):
     n_gat = len(gumbels) // A
     assert len(gumbels) == A * n_gat and n_gat == T + 1 and len(selects) == T
 
-    # ---- the same runner body with the B200-native objects (INTEGRATION.md §1) ---------------------------------
+    # ---- the same runner body with the iplan_b200 objects (INTEGRATION.md §1) ---------------------------------
     import runners.ippo_parallel_runner as ref_runner_mod                      # staged reference module
     import copy
     gargs = copy.copy(args)

@@ -1,5 +1,5 @@
 """BASELINE.json configs[4] — GAT_Net.forward at hidden width 128, 16 slots (the synthetic GAT + GRU microbench):
-the CUDA path (iplan_b200/nova/gat128.py: library GEMMs + the tcgen05 recurrence with W_hh in tensor memory + the
+the CUDA path (iplan_b200/nova/gat128.py: library GEMMs + the wgmma recurrence with W_hh in shared memory + the
 attention / gate kernels) against the CPU oracle's ``gat_forward`` (oracle/iplan_oracle.py, generic in the widths, pinned
 to the reference's GAT_Net by tests/test_oracle_golden.py) with explicit Gumbel noise.  Tolerance 1e-4 (north_star)."""
 import os
@@ -16,7 +16,7 @@ if ROOT not in sys.path:
 
 @pytest.mark.parametrize("A,items", [(2, 5), (3, 64)])
 def test_gat128_vs_oracle(A, items):
-    """Odd / even item counts (two items are in flight per CTA), several agent-nets; dl, hard gates and the output."""
+    """Odd / even item counts, several agent-nets; dl, hard gates and the output."""
     if not torch.cuda.is_available():
         pytest.skip("needs a CUDA device")
     from iplan_b200.nova.gat128 import GAT128, H, N

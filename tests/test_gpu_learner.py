@@ -176,14 +176,14 @@ def test_train_vs_oracle_highway_shape():
 
 
 @pytest.mark.parametrize("shape", [(2, 300, 272), (1, 128, 2485), (3, 1000, 2485)])
-def test_fc1_tcgen05_matches_mma_sync_and_fp64(shape):
-    """The tcgen05 / TMEM / TMA fc1 forward and backward (csrc/fc1_tc5.cu) against the mma.sync kernels and an
-    fp64 reference on the same operands: ragged rows, ragged K (Fp = 288 is not a multiple of the 64-wide k-block)."""
+def test_fc1_matches_fp64(shape):
+    """The fc1 forward and backward tensor-core products (csrc/fc1_mma.cu) against an fp64 reference on the same operands:
+    ragged rows, ragged K (Fp = 288 is not a multiple of the 64-wide k-block)."""
     if not torch.cuda.is_available():
         pytest.skip("needs a CUDA device")
     import importlib.util
     spec = importlib.util.spec_from_file_location(
-        "check_fc1_tc5", os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tools", "check_fc1_tc5.py"))
+        "check_fc1", os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tools", "check_fc1.py"))
     mod = importlib.util.module_from_spec(spec)
     spec.loader.exec_module(mod)
     assert mod.run(*shape, reps=1) < 1e-5
