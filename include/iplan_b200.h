@@ -243,6 +243,23 @@ int iplan_beh_learn(const float* enc_params, int64_t enc_stride, const float* de
                     uint64_t seed, uint64_t counter, float p_drop, float soft_coef, float thres_small_variation,
                     int n_agents, int n_eps, int n_steps, int n_slots, int obs_dim, int latent_dim, int hist_len, void* stream);
 
+/* ---- Behavior_policy.learn of the hard-update variant (iPLAN-Hard; nova/behavior_policy.py:119-215) ------------------
+ * Arithmetic specified by tools/beh_hard_oracle.py::behavior_learn_hard_agent.  The register-tiled kernels of
+ * iplan_beh_learn for any window geometry: window row w (0 <= w < W) of position j (0 <= j < n_pos) is
+ * win_first + j * win_step + w (rows below 0 are zeros), its target row is W later and the mask is read at the target
+ * row.  iplan_beh_learn is the geometry (1, 1 - W) with n_pos = T - 1 - W; the hard update is (W, 0) with
+ * n_pos = T / W - 1 and the mask lagged by one window on the host (the reference weighs target row t with mask[t - W],
+ * :144-152).  Rejects, before any launch, n_pos < 1, win_step < 1 and target rows outside [0, n_steps).
+ * scale [A][n_pos], keep NULL or uint8 [A][B][n_pos][N][W][64]; scratch: iplan_beh_learn_tile_scratch_floats (whatever
+ * iplan_beh_learn_set_impl selected).  soft_coef = 1 for the hard update (latent_j = the encoder's soft-max output). */
+int64_t iplan_beh_learn_tile_scratch_floats(int n_agents, int n_eps, int n_pos, int n_slots, int obs_dim, int latent_dim, int hist_len);
+int iplan_beh_learn_windows(const float* enc_params, int64_t enc_stride, const float* dec_params, int64_t dec_stride,
+                            float* g_enc, float* g_dec, const float* hist, const float* mask, const float* scale, const uint8_t* keep,
+                            float* b_loss, float* s_loss, float* scratch, int64_t scratch_floats,
+                            uint64_t seed, uint64_t counter, float p_drop, float soft_coef, float thres_small_variation,
+                            int n_agents, int n_eps, int n_steps, int n_slots, int obs_dim, int latent_dim, int hist_len,
+                            int n_pos, int win_step, int win_first, void* stream);
+
 /* ==== IPPO learner (IPPOLearner.train, learners/ippo_learner.py:227-317) ===============
  * All agents are processed together.  Agent a's input matrix is X_a[rows][ldx] with
  * rows = n_eps*(T+1), row (b,t) at index b*(T+1)+t — the packed EpisodeBatch layout.

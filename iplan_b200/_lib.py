@@ -62,6 +62,9 @@ _SIGNATURES = {
     "iplan_beh_learn_set_impl": (_i, [_i]),
     "iplan_beh_learn": (_i, [_p, _i64, _p, _i64, _p, _p, _p, _p, _p, _p, _p, _p, _p, _i64, _u64, _u64, _f, _f, _f,
                              _i, _i, _i, _i, _i, _i, _i, _p]),
+    "iplan_beh_learn_tile_scratch_floats": (_i64, [_i, _i, _i, _i, _i, _i, _i]),
+    "iplan_beh_learn_windows": (_i, [_p, _i64, _p, _i64, _p, _p, _p, _p, _p, _p, _p, _p, _p, _i64, _u64, _u64, _f, _f, _f,
+                                     _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _p]),
     "iplan_learner_row_stats": (_i, [_p, _i64, _i, _i, _i64, _i, _p, _p]),
     "iplan_learner_x_split": (_i, [_p, _i64, _p, _p, _p]),
     "iplan_learner_fc1_forward": (_i, [_p, _i64, _p, _i64, _p, _p, _i64, _i, _i, _i64, _i, _p, _p, _p, _p, _p, _p, _p]),

@@ -251,7 +251,11 @@ struct Args {
     float* slab;              // [A][tiles][W][slab rows][64]   the window being back-propagated
     uint64_t seed, counter; float p_drop, coef, thres, stab_scale;
     int B, T, N, o, L, W, n_pos, tiles;
+    int win_step, win_first;  // window row w of position j = win_first + j * win_step + w (rows < 0 read as zeros);
+                              // its target row is W later.  Soft update: (1, 1 - W), hard update: (W, 0)
 };
+
+__device__ __forceinline__ int win_row(const Args& a, int j, int w) { return a.win_first + j * a.win_step + w; }
 
 constexpr int HE = IPLAN_HID, HD = IPLAN_RNN;
 // slab rows per step
@@ -353,7 +357,7 @@ __device__ float* enc_window(float* sm, const Args& a, const float* __restrict__
     float* xin = sm + EncSmem::XIN; float* us = sm + EncSmem::U;
     float* hnext = hcur == sm + EncSmem::HA ? sm + EncSmem::HB : sm + EncSmem::HA;
     for (int w = 0; w < a.W; ++w) {
-        load_hist_rows(xin, hist, ci, j - a.W + 1 + w, a.N, a.o);
+        load_hist_rows(xin, hist, ci, win_row(a, j, w), a.N, a.o);
         __syncthreads();
         input_layer<HE>(us, xin, sm + EncSmem::LW, sm + EncSmem::LB, a.o, t);
         __syncthreads();
@@ -517,7 +521,7 @@ __global__ void __launch_bounds__(NT, 2) enc_bwd_kernel(Args a) {
             gate_derivs<HE>(DG, t, deh, sl + E_R * RC, sl + E_Z * RC, sl + E_N * RC, sl + E_GH * RC, hp_g, dhz);
             tile_g2s(us, sl + E_U * RC, HE);
             tile_g2s(P, hp_g, HE);
-            load_hist_rows(xin, hist, ci, j - W + 1 + w, a.N, o);
+            load_hist_rows(xin, hist, ci, win_row(a, j, w), a.N, o);
             __syncthreads();
             gru_dw<HE>(DG, us, P, t, aih, ahh);
             float du[4][2], dhp[4][2];
@@ -596,7 +600,7 @@ __device__ __forceinline__ void keep_bits(const Args& a, const ChainInfo* ci, co
 
 // decoder input tile of (position j, step w): rows 0..o-1 the window row, rows o..o+L-1 latent_j
 __device__ __forceinline__ void dec_input(float* xin, const Args& a, const float* __restrict__ hist, const float* __restrict__ lat_j, const ChainInfo* ci, int j, int w) {
-    load_hist_rows(xin, hist, ci, j - a.W + 1 + w, a.N, a.o);
+    load_hist_rows(xin, hist, ci, win_row(a, j, w), a.N, a.o);
     for (int idx = threadIdx.x; idx < a.L * RC; idx += NT) {
         const int l = idx >> 6, c = idx & 63;
         xin[(a.o + l) * RS + c] = lat_j[idx];
@@ -660,13 +664,14 @@ __device__ float* dec_window(float* sm, const Args& a, const float* __restrict__
         if (tid < RC) {
             const int c = tid;
             const bool valid = ci->gid[c] >= 0;
+            const int tr = win_row(a, j, w) + a.W;              // target row (the mask is read at the same row)
             float e2 = 0.0f;
             for (int oo = 0; oo < o; ++oo) {
                 const float pv = sm[DecSmem::OB + oo] + ((part[oo * RS + c] + part[(8 + oo) * RS + c]) + (part[(16 + oo) * RS + c] + part[(24 + oo) * RS + c]));
                 if (STORE) sl[(D_P + oo) * RC + c] = pv;
                 if (LOSS && valid) {
-                    const float nx = hist[ci->hoff[c] + (int64_t)(j + 1 + w) * a.N * o + oo];
-                    bl += fabsf(nx - pv) * mask[ci->moff[c] + j + 1 + w] * scale_j;
+                    const float nx = hist[ci->hoff[c] + (int64_t)tr * a.N * o + oo];
+                    bl += fabsf(nx - pv) * mask[ci->moff[c] + tr] * scale_j;
                     const float dcur = xin[oo * RS + c] - pv;
                     e2 = fmaf(dcur, dcur, e2);
                 }
@@ -754,8 +759,9 @@ __global__ void __launch_bounds__(NT, 1) dec_kernel(Args a) {
                 const int oo = idx >> 6, c = idx & 63;
                 float v = 0.0f;
                 if (oo < o && ci->gid[c] >= 0) {
-                    const float e = sl[(D_P + oo) * RC + c] - hist[ci->hoff[c] + (int64_t)(j + 1 + w) * a.N * o + oo];
-                    v = (e > 0.0f ? 1.0f : (e < 0.0f ? -1.0f : 0.0f)) * mask[ci->moff[c] + j + 1 + w] * scale[j];
+                    const int tr = win_row(a, j, w) + W;          // target row (the mask is read at the same row)
+                    const float e = sl[(D_P + oo) * RC + c] - hist[ci->hoff[c] + (int64_t)tr * a.N * o + oo];
+                    v = (e > 0.0f ? 1.0f : (e < 0.0f ? -1.0f : 0.0f)) * mask[ci->moff[c] + tr] * scale[j];
                 }
                 dpr[oo * RS + c] = v;
             }
@@ -867,16 +873,16 @@ extern "C" int64_t iplan_beh_learn_tile_scratch_floats(int n_agents, int n_eps, 
     return (int64_t)n_agents * tiles * iplan::blt::per_tile_floats(n_pos, latent_dim, hist_len);
 }
 
-extern "C" int iplan_beh_learn_tile(const float* enc_params, int64_t enc_stride, const float* dec_params, int64_t dec_stride,
-                                    float* g_enc, float* g_dec, const float* hist, const float* mask, const float* scale, const uint8_t* keep,
-                                    float* b_loss, float* s_loss, float* scratch, int64_t scratch_floats,
-                                    uint64_t seed, uint64_t counter, float p_drop, float soft_coef, float thres_small_variation,
-                                    int n_agents, int n_eps, int n_steps, int n_slots, int obs_dim, int latent_dim, int hist_len, void* stream) {
+// the three launches for window positions j = 0 .. n_pos-1 of geometry (win_step, win_first); the caller checked n_pos and the geometry
+static int beh_learn_tiled(const float* enc_params, int64_t enc_stride, const float* dec_params, int64_t dec_stride,
+                           float* g_enc, float* g_dec, const float* hist, const float* mask, const float* scale, const uint8_t* keep,
+                           float* b_loss, float* s_loss, float* scratch, int64_t scratch_floats,
+                           uint64_t seed, uint64_t counter, float p_drop, float soft_coef, float thres_small_variation,
+                           int n_agents, int n_eps, int n_steps, int n_slots, int obs_dim, int latent_dim, int hist_len,
+                           int n_pos, int win_step, int win_first, void* stream) {
     using namespace iplan;
     using namespace iplan::blt;
     IPLAN_REQUIRE(enc_params && dec_params && g_enc && g_dec && hist && mask && scale && b_loss && s_loss && scratch, "beh_learn: null pointer");
-    const int n_pos = n_steps - 1 - hist_len;
-    IPLAN_REQUIRE(n_pos > 0, "beh_learn: episode of %d steps is shorter than the window of %d", n_steps, hist_len);
     IPLAN_REQUIRE(obs_dim > 0 && obs_dim <= 8 && latent_dim > 0 && latent_dim <= 8 && (latent_dim & 1) == 0 && n_slots > 0, "beh_learn: obs_dim <= 8 and an even latent_dim <= 8 are built (got %d, %d)", obs_dim, latent_dim);
     IPLAN_REQUIRE(n_agents > 0 && n_eps > 0 && p_drop >= 0.f && p_drop < 1.f, "beh_learn: bad arguments");
     IPLAN_REQUIRE((int64_t)n_eps * n_steps * n_slots * obs_dim < (int64_t)1 << 31, "beh_learn: history block of one agent exceeds 2^31 elements");
@@ -897,6 +903,7 @@ extern "C" int iplan_beh_learn_tile(const float* enc_params, int64_t enc_stride,
     a.seed = seed; a.counter = counter; a.p_drop = p_drop; a.coef = soft_coef; a.thres = thres_small_variation;
     a.stab_scale = 1.0f / ((float)n_eps * (float)hist_len * (float)n_pos);
     a.B = n_eps; a.T = n_steps; a.N = n_slots; a.o = obs_dim; a.L = latent_dim; a.W = hist_len; a.n_pos = n_pos; a.tiles = tiles;
+    a.win_step = win_step; a.win_first = win_first;
     const size_t smem_e = sizeof(float) * (size_t)EncSmem::TOTAL, smem_d = sizeof(float) * (size_t)DecSmem::TOTAL;
     static_assert(sizeof(float) * DecSmem::TOTAL <= 227 * 1024, "decoder tile does not fit in shared memory");
     static bool configured = false;
@@ -913,4 +920,38 @@ extern "C" int iplan_beh_learn_tile(const float* enc_params, int64_t enc_stride,
     enc_bwd_kernel<<<grid, NT, smem_e, (cudaStream_t)stream>>>(a);
     count_launch(3);
     return check_launch("beh_learn_tile");
+}
+
+// soft update (reference nova/stable_behavior_policy.py:206-240): one position per step, the window ending at step j
+extern "C" int iplan_beh_learn_tile(const float* enc_params, int64_t enc_stride, const float* dec_params, int64_t dec_stride,
+                                    float* g_enc, float* g_dec, const float* hist, const float* mask, const float* scale, const uint8_t* keep,
+                                    float* b_loss, float* s_loss, float* scratch, int64_t scratch_floats,
+                                    uint64_t seed, uint64_t counter, float p_drop, float soft_coef, float thres_small_variation,
+                                    int n_agents, int n_eps, int n_steps, int n_slots, int obs_dim, int latent_dim, int hist_len, void* stream) {
+    using namespace iplan;
+    const int n_pos = n_steps - 1 - hist_len;
+    IPLAN_REQUIRE(n_pos > 0, "beh_learn: episode of %d steps is shorter than the window of %d", n_steps, hist_len);
+    return beh_learn_tiled(enc_params, enc_stride, dec_params, dec_stride, g_enc, g_dec, hist, mask, scale, keep, b_loss, s_loss, scratch,
+                           scratch_floats, seed, counter, p_drop, soft_coef, thres_small_variation, n_agents, n_eps, n_steps, n_slots,
+                           obs_dim, latent_dim, hist_len, n_pos, 1, 1 - hist_len, stream);
+}
+
+// any window geometry, e.g. the hard update (reference nova/behavior_policy.py:141-181): non-overlapping windows (W, 0)
+extern "C" int iplan_beh_learn_windows(const float* enc_params, int64_t enc_stride, const float* dec_params, int64_t dec_stride,
+                                       float* g_enc, float* g_dec, const float* hist, const float* mask, const float* scale, const uint8_t* keep,
+                                       float* b_loss, float* s_loss, float* scratch, int64_t scratch_floats,
+                                       uint64_t seed, uint64_t counter, float p_drop, float soft_coef, float thres_small_variation,
+                                       int n_agents, int n_eps, int n_steps, int n_slots, int obs_dim, int latent_dim, int hist_len,
+                                       int n_pos, int win_step, int win_first, void* stream) {
+    using namespace iplan;
+    IPLAN_REQUIRE(n_pos >= 1 && hist_len >= 1 && win_step >= 1, "beh_learn_windows: need n_pos >= 1, hist_len >= 1, win_step >= 1 (got %d, %d, %d)",
+                  n_pos, hist_len, win_step);
+    // window rows below 0 are zero padding; every target row (window row + W) must be a step of the episode
+    const int64_t first_target = (int64_t)win_first + hist_len;
+    const int64_t last_target = (int64_t)win_first + (int64_t)(n_pos - 1) * win_step + 2 * (int64_t)hist_len - 1;
+    IPLAN_REQUIRE(first_target >= 0 && last_target < n_steps, "beh_learn_windows: target rows [%lld, %lld] outside the episode of %d steps",
+                  (long long)first_target, (long long)last_target, n_steps);
+    return beh_learn_tiled(enc_params, enc_stride, dec_params, dec_stride, g_enc, g_dec, hist, mask, scale, keep, b_loss, s_loss, scratch,
+                           scratch_floats, seed, counter, p_drop, soft_coef, thres_small_variation, n_agents, n_eps, n_steps, n_slots,
+                           obs_dim, latent_dim, hist_len, n_pos, win_step, win_first, stream);
 }

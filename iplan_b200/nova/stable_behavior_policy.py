@@ -183,8 +183,27 @@ class Behavior_policy:
         j = torch.arange(n_pos, device=dev)
         msum = (cs[:, j + W] - cs[:, j]) * (N * o)                       # unmasked elements of the next-window at position j
         scale = ((o * N) / (msum + 1e-10) / n_pos).contiguous()
+        bl, sl, norms = self._learn_step(hist_a, mask_a, scale, n_pos)
+        behavior_loss = [np.asarray(float(bl[i]), dtype=np.float32) for i in range(A)]
+        stability_loss = [np.asarray(float(sl[i]), dtype=np.float32) for i in range(A)]
+        total_loss = [np.asarray(float(bl[i]), dtype=np.float32) for i in range(A)]          # penalty = 0
+        self._log(t_env, dict(behavior_loss=float(bl.sum()), stability_loss=float(sl.sum()), behavior_total=float(bl.sum()),
+                              behavior_encoder_grad_norm=float(norms[:, 0].sum()), behavior_decoder_grad_norm=float(norms[:, 1].sum())))
+        return behavior_loss, stability_loss, total_loss
+
+    def _learn_step(self, hist_a, mask_a, scale, n_pos, windows=None):
+        """Loss and gradients of every agent-net (one native call), then per agent-net the separately clipped encoder and
+        decoder gradients and one Adam step over both.  hist_a [A,B,T,N,o], mask_a [A,B,T] (read at the target row),
+        scale [A,n_pos].  ``windows = (win_step, win_first)`` selects a window geometry (iplan_beh_learn_windows); None is
+        the soft update's sliding window (iplan_beh_learn).  Returns (behavior loss [A], stability loss [A], clip norms
+        [A,8]: column 0 encoder, 1 decoder) on the host."""
+        args, dev = self.args, self.device
+        A, N, o, L, W = self.n_agents, self.max_vehicle_num, args.obs_shape_single, self.latent_dim, self.max_history_len
+        B, T = hist_a.shape[1], hist_a.shape[2]
+        lib, st, ptr = _lib.lib, _lib.stream(), _lib.ptr
         w = self._learn_state()
-        need = _lib.lib.iplan_beh_learn_scratch_floats(A, B, n_pos, N, o, L, W)
+        scratch_floats = lib.iplan_beh_learn_scratch_floats if windows is None else lib.iplan_beh_learn_tile_scratch_floats
+        need = scratch_floats(A, B, n_pos, N, o, L, W)
         if w["scratch"] is None or w["scratch"].numel() < need:
             w["scratch"] = torch.empty(need, device=dev)
         w["g_enc"].zero_(); w["g_dec"].zero_(); w["stats"].zero_()
@@ -194,12 +213,14 @@ class Behavior_policy:
         if keep is not None:
             keep = keep.to(dev, torch.uint8).contiguous()
             assert tuple(keep.shape) == (A, B, n_pos, N, W, args.decoder_rnn_dim), keep.shape
-        lib, st, ptr = _lib.lib, _lib.stream(), _lib.ptr
-        _lib.check(lib.iplan_beh_learn(
-            ptr(self.stack.flat), self.stack.stride(), ptr(self.dec_stack.flat), self.dec_stack.stride(), ptr(w["g_enc"]), ptr(w["g_dec"]),
-            ptr(hist_a), ptr(mask_a), ptr(scale), ptr(keep), ptr(b_loss), ptr(s_loss), ptr(w["scratch"]), w["scratch"].numel(),
-            self.seed, self.learn_calls, float(args.decoder_dropout), float(self.soft_update_coef), float(args.thres_small_variation),
-            A, B, T, N, o, L, W, st), "beh_learn")
+        common = (ptr(self.stack.flat), self.stack.stride(), ptr(self.dec_stack.flat), self.dec_stack.stride(), ptr(w["g_enc"]), ptr(w["g_dec"]),
+                  ptr(hist_a), ptr(mask_a), ptr(scale), ptr(keep), ptr(b_loss), ptr(s_loss), ptr(w["scratch"]), w["scratch"].numel(),
+                  self.seed, self.learn_calls, float(args.decoder_dropout), float(self.soft_update_coef), float(args.thres_small_variation),
+                  A, B, T, N, o, L, W)
+        if windows is None:
+            _lib.check(lib.iplan_beh_learn(*common, st), "beh_learn")
+        else:
+            _lib.check(lib.iplan_beh_learn_windows(*common, n_pos, int(windows[0]), int(windows[1]), st), "beh_learn_windows")
         self.learn_calls += 1
         self.last_grads = dict(enc=w["g_enc"].clone(), dec=w["g_dec"].clone())       # raw (unclipped) gradients, for parity checks
         w["step"] += 1
@@ -208,16 +229,13 @@ class Behavior_policy:
             _lib.check(lib.iplan_learner_adam(ptr(stack.flat), ptr(g), ptr(m), ptr(v), ptr(ones), ptr(w["sq"]), stack.stride(),
                                               stack.total, A, float(args.lr_behavior), 0.9, 0.999, float(args.optim_eps), w["step"],
                                               float(args.max_grad_norm), 1.0, ptr(w["stats"]), col, st), "adam")
-        bl, sl, norms = b_loss.cpu(), s_loss.cpu(), w["stats"].cpu()
-        behavior_loss = [np.asarray(float(bl[i]), dtype=np.float32) for i in range(A)]
-        stability_loss = [np.asarray(float(sl[i]), dtype=np.float32) for i in range(A)]
-        total_loss = [np.asarray(float(bl[i]), dtype=np.float32) for i in range(A)]          # penalty = 0
-        self.train_info = dict(behavior_loss=float(bl.sum()), stability_loss=float(sl.sum()), behavior_total=float(bl.sum()),
-                               behavior_encoder_grad_norm=float(norms[:, 0].sum()), behavior_decoder_grad_norm=float(norms[:, 1].sum()))
-        if self.logger is not None and t_env - self.log_stats_t >= getattr(args, "learner_log_interval", 0):
+        return b_loss.cpu(), s_loss.cpu(), w["stats"].cpu()
+
+    def _log(self, t_env, train_info):
+        self.train_info = train_info
+        if self.logger is not None and t_env - self.log_stats_t >= getattr(self.args, "learner_log_interval", 0):
             for k, v in self.train_info.items():
                 self.logger.log_stat(self.log_prefix + k, v, t_env)
-        return behavior_loss, stability_loss, total_loss
 
     # ---- checkpoints (reference :282-312) -------------------------------------------
     def save_models(self, path):
