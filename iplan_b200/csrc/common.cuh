@@ -148,8 +148,11 @@ __device__ __forceinline__ uint4 philox4x32(uint4 ctr, uint2 key) {
     }
     return ctr;
 }
-// uniform in (0,1): never 0 or 1
-__device__ __forceinline__ float u01(uint32_t x) { return ((x >> 8) + 0.5f) * (1.0f / 16777216.0f); }
+// uniform in (0,1), never 0 or 1: the top 24 bits plus one half, scaled by 2^-24, capped at the largest float below 1.
+// From 2^23 up the sum rounds to even in fp32, and 2^24 - 1 + 0.5 rounds to 2^24, i.e. exactly 1.0 (then log(1 - u) is
+// -inf); the cap maps that one input to 1 - 2^-24 and leaves every other value, and so every noise stream, unchanged.
+// oracle/philox.py restates this bit for bit.
+__device__ __forceinline__ float u01(uint32_t x) { return fminf(((x >> 8) + 0.5f) * (1.0f / 16777216.0f), 0x1.fffffep-1f); }
 #endif  // __CUDACC__
 
 }  // namespace iplan

@@ -455,7 +455,14 @@ __global__ void __launch_bounds__(CTRL_THREADS, 1) controller_step_kernel(CtrlAr
                     if (lane >= o) cdf += t;
                 }
                 const unsigned m = __ballot_sync(0xffffffffu, lane < nA && uu >= cdf);
-                action = min(__popc(m), nA - 1);
+                // Never return an action of probability 0 (masked, or underflowed in the soft-max).  When uu is at or
+                // above the last cdf (uu = 1, or the fp32 sum of the probabilities falls short of 1), or lands on a
+                // zero-width step, take the last action with pr > 0 at or below the inverse-CDF choice.  nz is never
+                // 0: the largest logit has pr = 1 / den > 0.
+                const unsigned nz = __ballot_sync(0xffffffffu, lane < nA && pr > 0.0f);
+                const int pick = min(__popc(m), nA - 1);
+                const unsigned below = nz & (0xffffffffu >> (31 - pick));
+                action = below ? 31 - __clz(below) : __ffs(nz) - 1;
             }
             const float lp_a = __shfl_sync(0xffffffffu, lp, action);
             if (live) {

@@ -79,8 +79,8 @@ def gat_forward(p, obs, h_prev, gumbel, tau=0.01, return_parts=False):
         b_hh = p["hard_bi_GRU.bias_hh_l0" + sfx]
         ego = enc @ w_ih[:, :H].t() + b_ih                                       # [B, N, 3H]
         nbr = enc @ w_ih[:, H:].t()                                              # [B, N, 3H]
-        h = torch.zeros(B, N, H)                                                 # :78
-        out = torch.empty(B, N, N - 1, H)
+        h = torch.zeros(B, N, H, dtype=obs.dtype)                                # :78
+        out = torch.empty(B, N, N - 1, H, dtype=obs.dtype)
         for s in order:
             gi = ego + nbr[:, idx[:, s], :]
             h = gru_cell(gi, h, w_hh, b_hh)
@@ -151,13 +151,14 @@ def gat_forward_loops(p, obs, h_prev, gumbel, tau=0.01):
 
 
 def gat_latent_update(gat_params, history_single, encoder_hidden, behavior_latent, gumbel,
-                      loops=False):
+                      loops=False, dtype=torch.float32):
     """a1  Prediction_policy.GAT_latent_update (nova/prediction_policy.py:92-118).
     history_single [B,A,N,o], encoder_hidden [B,A,N,D], behavior_latent [B,A,N,L],
-    gumbel [A,B,N,N-1,2] -> [B,A,N,D]."""
-    hs = torch.as_tensor(history_single, dtype=torch.float32)
-    eh = torch.as_tensor(encoder_hidden, dtype=torch.float32)
-    bl = torch.as_tensor(behavior_latent, dtype=torch.float32)
+    gumbel [A,B,N,N-1,2] -> [B,A,N,D], computed in ``dtype`` (the parameters must have it too)."""
+    hs = torch.as_tensor(history_single, dtype=dtype)
+    eh = torch.as_tensor(encoder_hidden, dtype=dtype)
+    bl = torch.as_tensor(behavior_latent, dtype=dtype)
+    gumbel = torch.as_tensor(gumbel, dtype=dtype)
     B, A, N, _ = hs.shape
     D = eh.shape[-1]
     fn = gat_forward_loops if loops else gat_forward
@@ -279,6 +280,18 @@ def critic_value(p, obs, h0):
     return v.squeeze(-1), h1
 
 
+def inverse_cdf(probs, u):
+    """Categorical sampling by inverse CDF: probs [R, n_act], u [R] -> the first action whose cdf exceeds u.  Like
+    torch.distributions.Categorical it never returns a zero-probability action: where u is at or above the last cdf
+    (u = 1, or the sum of the probabilities falls short of 1) it returns the last action with probability > 0."""
+    n = probs.shape[-1]
+    act = (u.view(-1, 1).to(probs.dtype) >= probs.cumsum(-1)).sum(-1).clamp(max=n - 1)
+    pos = torch.arange(n).expand_as(probs)
+    cand = torch.where((probs > 0) & (pos <= act.view(-1, 1)), pos, torch.full_like(pos, -1)).amax(-1)
+    first = torch.where(probs > 0, pos, torch.full_like(pos, n)).amin(-1)
+    return torch.where(cand >= 0, cand, first)
+
+
 def select_actions(actor_params, critic_params, inputs, avail, rnn_a, rnn_c,
                    test_mode=False, uniforms=None):
     """a5  DcntrlMAC.select_actions_ippo (controllers/dcntrl_controller.py:27-58) with
@@ -296,8 +309,7 @@ def select_actions(actor_params, critic_params, inputs, avail, rnn_a, rnn_c,
         if test_mode or uniforms is None:
             act = probs.argmax(dim=-1)                                           # mode()
         else:
-            cdf = probs.cumsum(-1)
-            act = (uniforms[:, a:a + 1] >= cdf).sum(-1).clamp(max=probs.shape[-1] - 1)
+            act = inverse_cdf(probs, uniforms[:, a])
         out["logits"].append(logits)
         out["actions"].append(act)
         out["logp"].append(logp_all.gather(-1, act.view(-1, 1)).squeeze(-1))
@@ -593,9 +605,9 @@ def behavior_learn_agent(enc_p, dec_p, history, mask, keep, args, opt=None):
     W, L = args.max_history_len, args.latent_dim
     e_tr = [enc_p[k].requires_grad_(True) for k in BEH_ENCODER_KEYS]
     d_tr = [dec_p[k].requires_grad_(True) for k in DECODER_KEYS]
-    latent = torch.zeros(B, N, L)
-    eh = torch.zeros(B * N, args.encoder_rnn_dim)
-    dh = torch.zeros(B * N, args.decoder_rnn_dim)
+    latent = torch.zeros(B, N, L, dtype=history.dtype)
+    eh = torch.zeros(B * N, args.encoder_rnn_dim, dtype=history.dtype)
+    dh = torch.zeros(B * N, args.decoder_rnn_dim, dtype=history.dtype)
     n_pos = T - 1 - W
     b_err, s_err = 0.0, 0.0
     for j in range(n_pos):

@@ -33,11 +33,10 @@ def test_whole_episode_device_runner_vs_oracle(B, sample):
     if not torch.cuda.is_available():
         pytest.skip("needs a CUDA device")
     from iplan_b200.runners.synthetic_runner import build_system
-    from oracle import iplan_oracle as O
     torch.set_num_threads(max(1, min(16, os.cpu_count() or 1)))
     sysm = build_system(n_envs=B, env="highway", hazard=0.01, seed=11 + B)
     a = sysm.args
-    A, N, T, W, nA = a.n_agents, a.max_vehicle_num, a.episode_limit, a.max_history_len, a.n_actions
+    A, N, T = a.n_agents, a.max_vehicle_num, a.episode_limit
     with torch.no_grad():                                   # non-degenerate policy head (the 0.01-gain init is ~uniform)
         for ag in sysm.mac.agents:
             ag.act.action_out.linear.weight.mul_(30.0)
@@ -59,8 +58,20 @@ def test_whole_episode_device_runner_vs_oracle(B, sample):
     batch, *_ = sysm.runner.run(test_mode=False)
     torch.cuda.synchronize()
     assert len(rec["gumbel"]) == T + 1 and len(rec["uniforms"]) == T
+    worst, flips = oracle_episode(sysm, batch, S, rec)
+    print(f"[episode B={B} envs {S}] worst |cuda - oracle| over {T} steps: " + " ".join(f"{k} {v:.2e}" for k, v in worst.items())
+          + f"; sampled actions differing: {flips} of {T * A * len(S)}")
+    assert flips <= 1
+    assert all(v < TOL for v in worst.values()), worst
 
-    # ---- the oracle on the sampled environments ------------------------------------------------------------
+
+def oracle_episode(sysm, batch, S, rec):
+    """The oracle stepping the episode ``sysm.runner.run`` just ran, for the environments S, fed the noise of every K1
+    call (rec["gumbel"][k]: [A, len(S), N, N-1, 2]) and K1c call (rec["uniforms"][t]: [A, len(S)]).  Returns the worst
+    |CUDA - oracle| per quantity and the number of sampled actions that differ."""
+    from oracle import iplan_oracle as O
+    a = sysm.args
+    A, N, T, W, nA = a.n_agents, a.max_vehicle_num, a.episode_limit, a.max_history_len, a.n_actions
     gat_p, beh_p = _params(sysm.prediction.stack), _params(sysm.behavior.stack)
     act_p, cri_p = _params(sysm.mac.actor_stack), _params(sysm.mac.critic_stack)
     hist = sysm.env.history[:, S].cpu()                     # [T+1, s, A, N, o]
@@ -107,10 +118,7 @@ def test_whole_episode_device_runner_vs_oracle(B, sample):
             att, beh, enc = att_new, torch.as_tensor(beh_new), torch.as_tensor(enc_new)
             worst["att"] = max(worst["att"], float((got["attention_latent"][:, t + 1] - att).abs().max()))
             worst["beh"] = max(worst["beh"], float((got["behavior_latent"][:, t + 1] - beh).abs().max()))
-    print(f"[episode B={B} envs {S}] worst |cuda - oracle| over {T} steps: " + " ".join(f"{k} {v:.2e}" for k, v in worst.items())
-          + f"; sampled actions differing: {flips} of {T * A * ns}")
-    assert flips <= 1
-    assert all(v < TOL for v in worst.values()), worst
+    return worst, flips
 
 
 def test_learner_vs_oracle_baseline_shape():

@@ -28,9 +28,9 @@ def behavior_learn_hard_agent(enc_p, dec_p, history, mask, keep, args, opt=None)
     e_tr = [enc_p[k].requires_grad_(True) for k in BEH_ENCODER_KEYS]
     d_tr = [dec_p[k].requires_grad_(True) for k in DECODER_KEYS]
     wins = history.reshape(B, n_win, W, N, o)
-    latent = torch.zeros(B, N, L)
-    eh = torch.zeros(B * N, args.encoder_rnn_dim)
-    dh = torch.zeros(B * N, args.decoder_rnn_dim)
+    latent = torch.zeros(B, N, L, dtype=history.dtype)
+    eh = torch.zeros(B * N, args.encoder_rnn_dim, dtype=history.dtype)
+    dh = torch.zeros(B * N, args.decoder_rnn_dim, dtype=history.dtype)
     preds = []
     for j in range(n_win - 1):
         curr = wins[:, j].permute(0, 2, 1, 3)                                         # [B, N, W, o]

@@ -19,6 +19,10 @@ from iplan_b200.config import make_args                                  # noqa:
 from iplan_b200.nova.prediction_policy import Prediction_policy          # noqa: E402
 from oracle import iplan_oracle as O                                     # noqa: E402
 
+# every raw gradient tensor against the oracle, relative to the tensor's largest entry: both recorded cases stay
+# below 1e-5 (worst 9.4e-6, on an NVIDIA H100 80GB HBM3); the kernel's float atomics vary the last bits run to run
+GRAD_REL = 2e-5
+
 
 def scheme_for(args):
     scheme = {
@@ -77,9 +81,9 @@ def run(case):
                 mine = flat[a, off:off + n].view(shape).cpu()
                 want = ref["grads"][name]
                 rel = float((mine - want).abs().max() / (want.abs().max() + 1e-12))
-                flagged = "" if rel < 1e-3 else "   <-- MISMATCH"
+                flagged = "" if rel < GRAD_REL else "   <-- MISMATCH"
                 print(f"    grad {kind}:{name:34s} rel {rel:.2e}{flagged}")
-                ok &= rel < 1e-3
+                ok &= rel < GRAD_REL
         after = {**{"gat:" + k: v for k, v in pol.pred_GAT[a].state_dict().items()}, **{"dec:" + k: v for k, v in pol.pred_decoder[a].state_dict().items()}}
         want = {**{"gat:" + k: v for k, v in g["gat_after"][a].items()}, **{"dec:" + k: v for k, v in g["dec_after"][a].items()}}
         worst = max(float((after[k].cpu() - want[k]).abs().max()) for k in want)
