@@ -26,6 +26,16 @@ extern "C" {
 
 #define IPLAN_ABI_VERSION 1
 #define IPLAN_MAX_SLOTS 64        /* N  (max_vehicle_num) supported by the GAT kernel */
+/* Joint limits below IPLAN_MAX_SLOTS, set by shared memory (227 KB per CTA on H100); each entry point rejects a larger
+ * shape before any launch:
+ *  - iplan_controller_step: feat_dim <= IPLAN_CTRL_MAX_FEAT.  The controller input is
+ *    N (obs_dim + 32 + latent_dim) + n_actions + n_agents wide, so at the Highway widths (obs_dim 5, latent_dim 8,
+ *    5 actions, 5 agents) a rollout runs at most N = 62 slots.
+ *  - iplan_pred_learn: n_slots <= IPLAN_PRED_LEARN_MAX_SLOTS, so Prediction_policy.learn trains at most 57 slots.
+ *  - iplan_behavior_step[_ex] and the register-tiled behaviour learner (iplan_beh_learn with the default implementation,
+ *    iplan_beh_learn_windows): obs_dim <= 7, so that the learner trains no encoder the rollout cannot run. */
+#define IPLAN_CTRL_MAX_FEAT 2800
+#define IPLAN_PRED_LEARN_MAX_SLOTS 57
 #define IPLAN_HID 32              /* GAT_hidden_dim == attention_dim == encoder_rnn_dim */
 #define IPLAN_RNN 64              /* rnn_hidden_dim == mlp_hidden_dim */
 #define IPLAN_MAX_ACT 8           /* n_actions upper bound */

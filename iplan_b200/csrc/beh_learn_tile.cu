@@ -883,7 +883,9 @@ static int beh_learn_tiled(const float* enc_params, int64_t enc_stride, const fl
     using namespace iplan;
     using namespace iplan::blt;
     IPLAN_REQUIRE(enc_params && dec_params && g_enc && g_dec && hist && mask && scale && b_loss && s_loss && scratch, "beh_learn: null pointer");
-    IPLAN_REQUIRE(obs_dim > 0 && obs_dim <= 8 && latent_dim > 0 && latent_dim <= 8 && (latent_dim & 1) == 0 && n_slots > 0, "beh_learn: obs_dim <= 8 and an even latent_dim <= 8 are built (got %d, %d)", obs_dim, latent_dim);
+    // obs_dim as the rollout's encoder step (K1b, behavior_step.cu) takes it: a module the rollout cannot run is not trained
+    IPLAN_REQUIRE(obs_dim > 0 && obs_dim <= 7, "beh_learn: obs_dim %d not in [1,7]", obs_dim);
+    IPLAN_REQUIRE(latent_dim > 0 && latent_dim <= 8 && (latent_dim & 1) == 0 && n_slots > 0, "beh_learn: an even latent_dim <= 8 is built (got %d)", latent_dim);
     IPLAN_REQUIRE(n_agents > 0 && n_eps > 0 && p_drop >= 0.f && p_drop < 1.f, "beh_learn: bad arguments");
     IPLAN_REQUIRE((int64_t)n_eps * n_steps * n_slots * obs_dim < (int64_t)1 << 31, "beh_learn: history block of one agent exceeds 2^31 elements");
     const int64_t need = iplan_beh_learn_tile_scratch_floats(n_agents, n_eps, n_pos, n_slots, obs_dim, latent_dim, hist_len);

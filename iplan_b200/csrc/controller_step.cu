@@ -479,6 +479,15 @@ __global__ void __launch_bounds__(CTRL_THREADS, 1) controller_step_kernel(CtrlAr
     }
 }
 
+// dynamic shared memory of controller_step_kernel at feature width F (the layout at the top of the kernel)
+constexpr size_t ctrl_smem_bytes(int F) {
+    const size_t ldh = (size_t)((F + 15) & ~15) + 8;
+    const size_t stage = std::max((size_t)2 * CTRL_ROWS * ldh * 2, (size_t)4 * CTRL_ROWS * 3 * R * sizeof(float));
+    return stage + ((size_t)2 * CTRL_ROWS * R + 4 * CTRL_ROWS * TAP + 2 * CTRL_ROWS) * sizeof(float);
+}
+static_assert(ctrl_smem_bytes(IPLAN_CTRL_MAX_FEAT) <= 227 * 1024 && ctrl_smem_bytes(IPLAN_CTRL_MAX_FEAT + 1) > 227 * 1024,
+              "IPLAN_CTRL_MAX_FEAT (include/iplan_b200.h) is not the largest feature width that fits");
+
 }  // namespace iplan
 
 extern "C" int iplan_controller_step(const float* actor_params, int64_t actor_stride,
@@ -511,9 +520,7 @@ extern "C" int iplan_controller_step(const float* actor_params, int64_t actor_st
     a.n_envs = n_envs; a.feat_dim = feat_dim; a.feat_ld = (feat_dim + 3) & ~3; a.n_actions = n_actions;
     static const int allow_vec = getenv("IPLAN_CTRL_VEC") ? atoi(getenv("IPLAN_CTRL_VEC")) : 1;
     a.allow_vec = allow_vec;
-    const size_t ldh = ((feat_dim + 15) & ~15) + 8;
-    const size_t stage = std::max((size_t)2 * CTRL_ROWS * ldh * 2, (size_t)4 * CTRL_ROWS * 3 * R * sizeof(float));
-    const size_t smem = stage + ((size_t)2 * CTRL_ROWS * R + 4 * CTRL_ROWS * TAP + 2 * CTRL_ROWS) * sizeof(float);
+    const size_t smem = ctrl_smem_bytes(feat_dim);
     IPLAN_REQUIRE(smem <= 227 * 1024, "controller_step: feat_dim %d needs %zu B of shared memory", feat_dim, smem);
     static size_t configured = 0;
     if (smem > configured) {

@@ -53,9 +53,13 @@ constexpr int KOFF = 36;        //   (8-byte aligned, (72 g + 2 t) mod 32 distin
 constexpr int WP = 64 + 8;      // attention-weight / V^T row pitch: K = 64 neighbour columns, zero padded
 __host__ __device__ inline size_t att_smem_floats(int N) {
     // s_vt (aliases s_x, s_we) | s_enc | s_xa | s_hp | s_gh | region { s_qk, s_dl, s_w }  (s_gi aliases the region)
+    // The score product (phase 5a) reads k rows up to the next multiple of 8 past N - 1, so the region holds at least
+    // that many q|k rows; below N = 4 this is more than s_qk + s_dl + s_w.
     const size_t region = (size_t)N * QKP + (size_t)N * (N - 1) + (size_t)N * WP;
+    const size_t qk_pad = (size_t)((N + 7) & ~7) * QKP;
     const size_t gru = (size_t)N * G3;
-    return (size_t)H * WP + 3 * (size_t)N * H + (size_t)N * G3 + (region > gru ? region : gru);
+    const size_t big = region > qk_pad ? region : qk_pad;
+    return (size_t)H * WP + 3 * (size_t)N * H + (size_t)N * G3 + (big > gru ? big : gru);
 }
 
 // volatile: the W_hh fragments are loop-invariant, and hoisting them out of the step loop would cost
@@ -391,8 +395,8 @@ __global__ void __launch_bounds__(GAT_THREADS, 2) gat_attend_kernel(GatArgs a) {
     __syncthreads();
 
     // ---- phase 5a: raw scores S[i][j] = q_i . k_j for every slot pair, on the tensor cores --------
-    // (columns are padded to a multiple of 8: rows of the q|k buffer past N-1 are whatever follows in shared memory;
-    //  those columns are never read)
+    // (columns are padded to a multiple of 8: rows of the q|k buffer past N-1 are whatever follows in shared memory,
+    //  inside the allocation (att_smem_floats); those columns are never read)
     dense32_mma<GAT_WARPS>(s_qk, QKP, N, s_qk + KOFF, QKP, nullptr, (N + 7) & ~7, s_w, WP, false, warp, lane);
     __syncthreads();
 

@@ -629,6 +629,8 @@ extern "C" int iplan_learner_row_stats(const float* X, int64_t x_stride_agent, i
 
 extern "C" int iplan_learner_tail(const iplan_learner_ctx* c, int train, void* stream_) {
     IPLAN_REQUIRE(c && c->Z1 && c->A1 && c->Z2 && c->A2 && c->GI && c->GH, "learner_tail: null work buffer");
+    IPLAN_REQUIRE(c->n_actions > 0 && c->n_actions <= IPLAN_MAX_ACT, "learner_tail: n_actions %d not in [1,%d]", c->n_actions, IPLAN_MAX_ACT);
+    IPLAN_REQUIRE(c->n_agents > 0 && c->n_eps > 0 && c->T1 > 0 && c->feat_dim > 0, "learner_tail: bad sizes");
     cudaStream_t st = (cudaStream_t)stream_;
     const int A = c->n_agents;
     const int64_t rows = (int64_t)c->n_eps * c->T1;

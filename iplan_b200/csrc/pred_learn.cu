@@ -572,6 +572,16 @@ extern "C" int64_t iplan_pdec_layout(int obs_dim, int64_t* offsets) {
     return L.total;
 }
 
+namespace iplan {
+// dynamic shared memory of pred_learn_kernel at N slots
+constexpr size_t pred_learn_smem_bytes(int N) {
+    return sizeof(float) * ((size_t)N * PIN + 2 * (size_t)N * PH + 3 * (size_t)N * (N - 1) + 2 * (size_t)N * PG
+                            + 2 * (size_t)N * PH + PG * 33 + 2 * (size_t)N * PH + 4 * (size_t)N * PG);
+}
+static_assert(pred_learn_smem_bytes(IPLAN_PRED_LEARN_MAX_SLOTS) <= 227 * 1024 && pred_learn_smem_bytes(IPLAN_PRED_LEARN_MAX_SLOTS + 1) > 227 * 1024,
+              "IPLAN_PRED_LEARN_MAX_SLOTS (include/iplan_b200.h) is not the largest slot count that fits");
+}  // namespace iplan
+
 extern "C" int64_t iplan_pred_learn_scratch_floats(int n_agents, int n_samples, int n_slots, int obs_dim, int pred_len) {
     const int64_t N = n_slots, pl = pred_len, o = obs_dim, H = IPLAN_HID, G = 3 * IPLAN_HID;
     const int64_t per = 2 * N * (N - 1) * H + pl * N * o + pl * N * H + (pl + 1) * N * H + pl * N * H + pl * N * o
@@ -599,10 +609,9 @@ extern "C" int iplan_pred_learn(const float* gat_params, int64_t gat_stride, con
     a.loss_sum = loss_sum; a.scratch = scratch; a.scratch_per_cta = need / ((int64_t)n_agents * n_samples);
     a.seed = seed; a.counter = counter; a.inv_tau = 1.0f / tau; a.p_drop = p_drop;
     a.P = n_samples; a.N = n_slots; a.o = obs_dim; a.L = latent_dim; a.pl = pred_len;
-    const int N = n_slots;
-    const size_t smem = sizeof(float) * ((size_t)N * PIN + 2 * (size_t)N * PH + 3 * (size_t)N * (N - 1) + 2 * (size_t)N * PG
-                                         + 2 * (size_t)N * PH + PG * 33 + 2 * (size_t)N * PH + 4 * (size_t)N * PG);
-    IPLAN_REQUIRE(smem <= 227 * 1024, "pred_learn: %zu B of shared memory", smem);
+    const size_t smem = pred_learn_smem_bytes(n_slots);
+    IPLAN_REQUIRE(smem <= 227 * 1024, "pred_learn: n_slots %d needs %zu B of shared memory (at most %d slots fit)", n_slots, smem,
+                  IPLAN_PRED_LEARN_MAX_SLOTS);
     static size_t configured = 0;
     if (smem > configured) {
         cudaError_t e = cudaFuncSetAttribute(pred_learn_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
