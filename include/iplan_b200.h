@@ -270,6 +270,48 @@ int iplan_beh_learn_windows(const float* enc_params, int64_t enc_stride, const f
                             int n_agents, int n_eps, int n_steps, int n_slots, int obs_dim, int latent_dim, int hist_len,
                             int n_pos, int win_step, int win_first, void* stream);
 
+/* ---- iPLAN-FC behaviour module (behavior_fully_connected: True; nova/behavior_FC_policy.py, nova/behavior_FC_net.py) ----
+ * Arithmetic specified by tools/beh_fc_oracle.py.  Encoder_3FC: K0 = hist_len * obs_dim -> E -> E -> L, tanh, tanh,
+ * soft-max.  LILI_Latent_Decoder: [window | latent] (K0 + L) -> Dh -> Dh -> K0, tanh, tanh, linear.  Shape limits, checked
+ * by both entry points before any launch (each names the violated limit in iplan_last_error()):
+ *   enc_hidden == IPLAN_BFC_ENC_HIDDEN, dec_hidden == IPLAN_BFC_DEC_HIDDEN (the widths the kernels are written for),
+ *   1 <= latent_dim <= IPLAN_BFC_MAX_LATENT, obs_dim >= 1, hist_len >= 1,
+ *   hist_len * obs_dim + latent_dim <= IPLAN_BFC_MAX_IN (the decoder input is one 64-wide row of the learn tile).
+ * Parameter layouts: the state_dict tensors (weight, bias of linear_1, linear_2, out) in order, pad-to-4 as above;
+ * iplan_bfc_layout(K0, E, L) for the encoder, iplan_bfcdec_layout(K0, L, Dh) for the decoder. */
+#define IPLAN_BFC_NTENSORS 6
+#define IPLAN_BFC_ENC_HIDDEN 32
+#define IPLAN_BFC_DEC_HIDDEN 64
+#define IPLAN_BFC_MAX_LATENT 8
+#define IPLAN_BFC_MAX_IN 64
+int64_t iplan_bfc_layout(int in_dim, int hidden, int latent_dim, int64_t* offsets);
+int64_t iplan_bfcdec_layout(int in_dim, int latent_dim, int hidden, int64_t* offsets);
+
+/* Behavior_policy.latent_update of iPLAN-FC (nova/behavior_FC_policy.py:80-106): lat_out [a][b][n][L] = the encoder's
+ * soft-max output for the node's window.  No hidden state and no soft update.  The window is read as by
+ * iplan_behavior_step_ex: win_stride_step == 0 -> `window` is [a][b][n][hist_len*obs_dim]; otherwise row w of a node is at
+ * window.ptr + (w - win_pad) * win_stride_step, rows w < win_pad are zeros. */
+int iplan_behavior_fc_step(const float* enc_params, int64_t param_stride,
+                           iplan_view window, int64_t win_stride_step, int win_pad, iplan_view lat_out,
+                           int n_envs, int n_agents, int n_slots, int obs_dim, int latent_dim, int hist_len, int enc_hidden,
+                           void* stream);
+
+/* Behavior_policy.learn of iPLAN-FC (nova/behavior_FC_policy.py:146-236), loss and gradients of every agent-net in one
+ * launch.  hist [A][B][T][N][o] (the batch without its last step, T = n_steps), positions j = 0 .. n_pos-1 with
+ * n_pos = T - 1 - hist_len (rejected when < 1).  Row (a, b, n, j): the decoder reads [window ending at j | latent_{j-1}]
+ * with latent_{j-1} = encoder(window ending at j-1), latent_{-1} = 0; its target is the window ending at j+1.
+ * b_loss[a] += scale * sum |target - prediction| and d loss / d prediction = -scale * sign(target - prediction), with
+ * scale = o N / (B N W o + 1e-10) / n_pos (the reference's termination mask has no effect, :135-140).  Gradients are
+ * ADDED into g_enc / g_dec (parameter layouts and strides); the sums across CTAs are added in a fixed order, so two calls
+ * with the same arguments give the same bits.  The 64-wide decoder products run on the tensor cores (split-f16
+ * mma.sync); the encoder products are FP32.  Per CTA, gradients are summed tile by tile in fp32; parity with a float64
+ * oracle (loss 1e-6, every gradient tensor 1e-5 relative) is tested at 8 envs x 90 steps x 5 agents x 55 slots, about
+ * 20 tiles per CTA, and the 512-env shape runs about 1300 tiles per CTA.  Clip + Adam: iplan_learner_adam. */
+int iplan_beh_fc_learn(const float* enc_params, int64_t enc_stride, const float* dec_params, int64_t dec_stride,
+                       float* g_enc, float* g_dec, const float* hist, float scale, float* b_loss,
+                       int n_agents, int n_eps, int n_steps, int n_slots, int obs_dim, int latent_dim, int hist_len,
+                       int enc_hidden, int dec_hidden, void* stream);
+
 /* ==== IPPO learner (IPPOLearner.train, learners/ippo_learner.py:227-317) ===============
  * All agents are processed together.  Agent a's input matrix is X_a[rows][ldx] with
  * rows = n_eps*(T+1), row (b,t) at index b*(T+1)+t — the packed EpisodeBatch layout.

@@ -65,6 +65,10 @@ _SIGNATURES = {
     "iplan_beh_learn_tile_scratch_floats": (_i64, [_i, _i, _i, _i, _i, _i, _i]),
     "iplan_beh_learn_windows": (_i, [_p, _i64, _p, _i64, _p, _p, _p, _p, _p, _p, _p, _p, _p, _i64, _u64, _u64, _f, _f, _f,
                                      _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _p]),
+    "iplan_bfc_layout": (_i64, [_i, _i, _i, _p]),
+    "iplan_bfcdec_layout": (_i64, [_i, _i, _i, _p]),
+    "iplan_behavior_fc_step": (_i, [_p, _i64, View, _i64, _i, View, _i, _i, _i, _i, _i, _i, _i, _p]),
+    "iplan_beh_fc_learn": (_i, [_p, _i64, _p, _i64, _p, _p, _p, _f, _p, _i, _i, _i, _i, _i, _i, _i, _i, _i, _p]),
     "iplan_learner_row_stats": (_i, [_p, _i64, _i, _i, _i64, _i, _p, _p]),
     "iplan_learner_x_split": (_i, [_p, _i64, _p, _p, _p]),
     "iplan_learner_fc1_forward": (_i, [_p, _i64, _p, _i64, _p, _p, _i64, _i, _i, _i64, _i, _p, _p, _p, _p, _p, _p, _p]),
@@ -296,7 +300,7 @@ def as_host(x, dtype=torch.float32):
 
 def layout(kind, *dims):
     """(total floats per agent, [offsets]) of a flat parameter buffer."""
-    n = {"gat": 20, "beh": 8, "actor": 22, "critic": 26, "pdec": 8, "bdec": 8}[kind]
+    n = {"gat": 20, "beh": 8, "actor": 22, "critic": 26, "pdec": 8, "bdec": 8, "bfc": 6, "bfcdec": 6}[kind]
     arr = (C.c_int64 * n)()
     fn = getattr(lib, f"iplan_{kind}_layout")
     total = fn(*dims, C.cast(arr, C.c_void_p))

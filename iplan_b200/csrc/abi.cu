@@ -84,6 +84,19 @@ extern "C" int64_t iplan_beh_layout(int obs_dim, int latent_dim, int64_t* off) {
     }
     return L.total;
 }
+static int64_t bfc_offsets(const iplan::BfcLayout& L, int64_t* off) {
+    if (off) {
+        const int64_t v[IPLAN_BFC_NTENSORS] = {L.w1, L.b1, L.w2, L.b2, L.w3, L.b3};
+        memcpy(off, v, sizeof(v));
+    }
+    return L.total;
+}
+extern "C" int64_t iplan_bfc_layout(int in_dim, int hidden, int latent_dim, int64_t* off) {
+    return bfc_offsets(iplan::bfc_layout(in_dim, hidden, latent_dim), off);
+}
+extern "C" int64_t iplan_bfcdec_layout(int in_dim, int latent_dim, int hidden, int64_t* off) {
+    return bfc_offsets(iplan::bfc_layout(in_dim + latent_dim, hidden, in_dim), off);
+}
 static int64_t trunk_offsets(const iplan::TrunkLayout& L, int64_t* off, bool critic) {
     if (off) {
         const int64_t v[22] = {L.ln0_w, L.ln0_b, L.fc1_w, L.fc1_b, L.ln1_w, L.ln1_b, L.fch_w, L.fch_b, L.lnh_w, L.lnh_b,

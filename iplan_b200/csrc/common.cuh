@@ -76,6 +76,20 @@ __host__ __device__ inline BehLayout beh_layout(int obs_dim, int latent_dim) {
     return L;
 }
 
+struct BfcLayout {      // nova/behavior_FC_net.py:6-37 (Encoder_3FC, Decoder_3FC), state_dict order
+    int64_t w1, b1, w2, b2, w3, b3, total;
+};
+__host__ __device__ inline BfcLayout bfc_layout(int in_dim, int hidden, int out_dim) {
+    BfcLayout L;
+    int64_t o = 0;
+    auto take = [&](int64_t n) { int64_t at = o; o = pad4(o + n); return at; };
+    L.w1 = take((int64_t)hidden * in_dim); L.b1 = take(hidden);
+    L.w2 = take((int64_t)hidden * hidden); L.b2 = take(hidden);
+    L.w3 = take((int64_t)out_dim * hidden); L.b3 = take(out_dim);
+    L.total = o;
+    return L;
+}
+
 // R_Actor / R_Critic trunk (utils/mappo_utils/mlp.py, rnn.py), state_dict order.
 struct TrunkLayout {
     int64_t ln0_w, ln0_b;            // base.feature_norm

@@ -57,6 +57,20 @@ def bdec_spec(obs_dim, latent_dim, hidden=64):
             ("decoder.out.weight", (obs_dim, hidden)), ("decoder.out.bias", (obs_dim,))]
 
 
+def bfc_spec(in_dim, hidden, latent_dim):
+    """Encoder_3FC (nova/behavior_FC_net.py:6-20): W*o -> hidden -> hidden -> latent, state_dict order."""
+    return [("linear_1.weight", (hidden, in_dim)), ("linear_1.bias", (hidden,)),
+            ("linear_2.weight", (hidden, hidden)), ("linear_2.bias", (hidden,)),
+            ("out.weight", (latent_dim, hidden)), ("out.bias", (latent_dim,))]
+
+
+def bfcdec_spec(in_dim, latent_dim, hidden):
+    """LILI_Latent_Decoder -> Decoder_3FC (nova/behavior_FC_net.py:23-60): W*o + latent -> hidden -> hidden -> W*o."""
+    return [("decoder.linear_1.weight", (hidden, in_dim + latent_dim)), ("decoder.linear_1.bias", (hidden,)),
+            ("decoder.linear_2.weight", (hidden, hidden)), ("decoder.linear_2.bias", (hidden,)),
+            ("decoder.out.weight", (in_dim, hidden)), ("decoder.out.bias", (in_dim,))]
+
+
 def trunk_spec(feat_dim):
     """MLPBase + RNNLayer (utils/mappo_utils/mlp.py:17-22,44-48; rnn.py:13-22)."""
     return [("base.feature_norm.weight", (feat_dim,)), ("base.feature_norm.bias", (feat_dim,)),
@@ -141,12 +155,12 @@ class AgentNet(nn.Module):
 
 
 class ParamStack:
-    """[A, total] fp32 buffer + per-agent AgentNet views; `kind` in gat|beh|actor|critic|pdec."""
+    """[A, total] fp32 buffer + per-agent AgentNet views; `kind` in gat|beh|actor|critic|pdec|bdec|bfc|bfcdec."""
 
     def __init__(self, kind, n_agents, dims, device="cpu"):
         self.kind, self.n_agents, self.dims = kind, n_agents, tuple(dims)
         self.spec = {"gat": gat_spec, "beh": beh_spec, "actor": actor_spec, "critic": critic_spec, "pdec": pdec_spec,
-                     "bdec": bdec_spec}[kind](*dims)
+                     "bdec": bdec_spec, "bfc": bfc_spec, "bfcdec": bfcdec_spec}[kind](*dims)
         self.total, self.offsets = _lib.layout(kind, *(dims[:2] if kind == "bdec" else dims))
         assert len(self.offsets) == len(self.spec)
         # initialise on the host (orthogonal init = QR: dozens of tiny launches on a GPU), then move
@@ -195,7 +209,7 @@ class ParamStack:
 
     def _init_tensor(self, name, p):
         k = self.kind
-        if k in ("gat", "beh", "pdec", "bdec"):
+        if k in ("gat", "beh", "pdec", "bdec", "bfc", "bfcdec"):
             # torch defaults: Linear U(+-1/sqrt(fan_in)); GRU/GRUCell U(+-1/sqrt(hidden))
             if "GRU" in name or name.startswith("rnn.") or ".rnn." in name:
                 hidden = dict(self.spec)["decoder.rnn.weight_hh_l0"][1] if k in ("pdec", "bdec") else H

@@ -79,11 +79,8 @@ class Behavior_policy:
         self.max_history_len = args.max_history_len
         self.latent_dim = args.latent_dim
         self.soft_update_coef = args.soft_update_coef
-        assert args.encoder_rnn_dim == 32 and args.num_encoder_layer == 1, "kernel K1b is built for E = 32, one layer"
-        self.stack = ParamStack("beh", self.n_agents, (args.obs_shape_single, args.latent_dim), device=self.device)
+        self._build_nets(args)
         self.behavior_encoder = self.stack.nets
-        # the reconstruction decoder of the auxiliary learner (reference :48-53): parameters and checkpoints only — ``learn`` is not built
-        self.dec_stack = ParamStack("bdec", self.n_agents, (args.obs_shape_single, args.latent_dim, args.decoder_rnn_dim), device=self.device)
         self.behavior_decoder = self.dec_stack.nets
         self._stage = None        # device staging buffers of the pipelined numpy entry point
         self._learn = None          # Adam moments / work buffers of learn()
@@ -93,6 +90,13 @@ class Behavior_policy:
         self.log_stats_t = -getattr(args, "learner_log_interval", 0) - 1
         self.behavior_optimizer = [_BehAdam(self, i) for i in range(self.n_agents)]
         self.debug_keep = None      # uint8 [A, B, n_pos, N, W, 64] explicit dropout draw for the next learn() (parity runs)
+
+    def _build_nets(self, args):
+        """Parameter stacks of the encoder (``self.stack``) and of the reconstruction decoder (``self.dec_stack``)."""
+        assert args.encoder_rnn_dim == 32 and args.num_encoder_layer == 1, "kernel K1b is built for E = 32, one layer"
+        self.stack = ParamStack("beh", self.n_agents, (args.obs_shape_single, args.latent_dim), device=self.device)
+        # the reconstruction decoder of the auxiliary learner (reference :48-53)
+        self.dec_stack = ParamStack("bdec", self.n_agents, (args.obs_shape_single, args.latent_dim, args.decoder_rnn_dim), device=self.device)
 
     # ---- device path: tensors laid out [A, B, N, *] ----------------------------------
     def behavior_step(self, window, hid_io, lat_prev, lat_out, win_stride_step=0, win_pad=0):
@@ -222,6 +226,15 @@ class Behavior_policy:
         else:
             _lib.check(lib.iplan_beh_learn_windows(*common, n_pos, int(windows[0]), int(windows[1]), st), "beh_learn_windows")
         self.learn_calls += 1
+        self._adam_step()
+        return b_loss.cpu(), s_loss.cpu(), w["stats"].cpu()
+
+    def _adam_step(self):
+        """After a learn kernel has filled g_enc / g_dec: keep the raw gradients in ``last_grads`` (parity checks), then
+        per agent-net clip the encoder and decoder gradients separately to max_grad_norm (pre-clip norms into stats
+        columns 0 and 1) and take one Adam step (lr_behavior) over both."""
+        args, w = self.args, self._learn_state()
+        lib, st, ptr, A = _lib.lib, _lib.stream(), _lib.ptr, self.n_agents
         self.last_grads = dict(enc=w["g_enc"].clone(), dec=w["g_dec"].clone())       # raw (unclipped) gradients, for parity checks
         w["step"] += 1
         for stack, g, m, v, ones, col in ((self.stack, w["g_enc"], w["m_enc"], w["v_enc"], w["ones_enc"], 0),
@@ -229,7 +242,6 @@ class Behavior_policy:
             _lib.check(lib.iplan_learner_adam(ptr(stack.flat), ptr(g), ptr(m), ptr(v), ptr(ones), ptr(w["sq"]), stack.stride(),
                                               stack.total, A, float(args.lr_behavior), 0.9, 0.999, float(args.optim_eps), w["step"],
                                               float(args.max_grad_norm), 1.0, ptr(w["stats"]), col, st), "adam")
-        return b_loss.cpu(), s_loss.cpu(), w["stats"].cpu()
 
     def _log(self, t_env, train_info):
         self.train_info = train_info

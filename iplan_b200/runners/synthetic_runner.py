@@ -283,7 +283,7 @@ def build_system(n_envs, env="highway", hazard=0.01, seed=112358, logger=None, *
     from ..controllers.dcntrl_controller import DcntrlMAC
     from ..learners.ippo_learner import IPPOLearner
     from ..nova.prediction_policy import Prediction_policy
-    from ..nova import behavior_policy, stable_behavior_policy
+    from ..nova import behavior_FC_policy, behavior_policy, stable_behavior_policy
     over = dict(batch_size_run=n_envs, buffer_size=n_envs, batch_size=n_envs - 1, use_cuda=True, device="cuda", seed=seed)
     if env != "highway" and "episode_limit" in overrides:
         overrides["episode_length"] = overrides.pop("episode_limit")
@@ -296,8 +296,13 @@ def build_system(n_envs, env="highway", hazard=0.01, seed=112358, logger=None, *
     probe = EpisodeBatch(scheme, groups, 1, 2, preprocess=preprocess, device="cpu")    # scheme incl. actions_onehot
     mac = DcntrlMAC(probe.scheme, groups, args)
     learner = IPPOLearner(mac, probe.scheme, logger, args)
-    # soft_update_enable: False is the iPLAN-Hard ablation (run_ippo.py:200-209)
-    behavior = (stable_behavior_policy if args.soft_update_enable else behavior_policy).Behavior_policy(args, logger)
+    # behavior_fully_connected: True is the iPLAN-FC ablation and wins over soft_update_enable, whose False is the
+    # iPLAN-Hard ablation (run_ippo.py:200-209)
+    if args.behavior_fully_connected:
+        behavior_module = behavior_FC_policy
+    else:
+        behavior_module = stable_behavior_policy if args.soft_update_enable else behavior_policy
+    behavior = behavior_module.Behavior_policy(args, logger)
     prediction = Prediction_policy(args, logger)
     runner.setup(scheme, groups, preprocess, mac, behavior, prediction)
 
