@@ -227,31 +227,37 @@ def build_inputs_train(agent_id, history, attention, behavior, actions_onehot, n
     bs, ts = history.shape[:2]
     slots = torch.cat([history, attention, behavior], dim=-1).reshape(bs, ts, -1)
     last = torch.cat([actions_onehot[:, 0:1], actions_onehot[:, :-1]], dim=1)
-    ident = torch.zeros(bs, ts, n_agents)
+    ident = torch.zeros(bs, ts, n_agents, dtype=history.dtype, device=history.device)
     ident[:, :, agent_id] = 1
     return torch.cat([slots, last, ident], dim=-1)
 
 
-def trunk_forward(p, obs, h0):
+def trunk_forward(p, obs, h0, taps=None):
     """MLPBase + RNNLayer (utils/mappo_utils/mlp.py:50-56, :24-28; rnn.py:24-78) for
     rows of length-1 sequences: obs [R, F], h0 [R, Rh] -> (features [R, Rh], h1 [R, Rh]).
-    ``fc_h`` exists in the state_dict but is never called (mlp.py:20-27)."""
+    ``fc_h`` exists in the state_dict but is never called (mlp.py:20-27).
+    ``taps`` (a dict) receives the GRU input ``a2`` [R, Rh], its projection ``gi`` [R, 3 Rh] and the two ReLUs'
+    inputs ``z1`` / ``z2`` and outputs ``r1`` / ``r2``."""
     x = F.layer_norm(obs, obs.shape[-1:], p["base.feature_norm.weight"],
                      p["base.feature_norm.bias"], 1e-5)
-    x = F.relu(x @ p["base.mlp.fc1.0.weight"].t() + p["base.mlp.fc1.0.bias"])
-    x = F.layer_norm(x, x.shape[-1:], p["base.mlp.fc1.2.weight"], p["base.mlp.fc1.2.bias"], 1e-5)
-    x = F.relu(x @ p["base.mlp.fc2.0.0.weight"].t() + p["base.mlp.fc2.0.0.bias"])
-    x = F.layer_norm(x, x.shape[-1:], p["base.mlp.fc2.0.2.weight"], p["base.mlp.fc2.0.2.bias"], 1e-5)
+    z1 = x @ p["base.mlp.fc1.0.weight"].t() + p["base.mlp.fc1.0.bias"]
+    r1 = F.relu(z1)
+    x = F.layer_norm(r1, r1.shape[-1:], p["base.mlp.fc1.2.weight"], p["base.mlp.fc1.2.bias"], 1e-5)
+    z2 = x @ p["base.mlp.fc2.0.0.weight"].t() + p["base.mlp.fc2.0.0.bias"]
+    r2 = F.relu(z2)
+    x = F.layer_norm(r2, r2.shape[-1:], p["base.mlp.fc2.0.2.weight"], p["base.mlp.fc2.0.2.bias"], 1e-5)
     gi = x @ p["rnn.rnn.weight_ih_l0"].t() + p["rnn.rnn.bias_ih_l0"]
+    if taps is not None:
+        taps.update(a2=x, gi=gi, z1=z1, r1=r1, z2=z2, r2=r2)
     h1 = gru_cell(gi, h0, p["rnn.rnn.weight_hh_l0"], p["rnn.rnn.bias_hh_l0"])
     feat = F.layer_norm(h1, h1.shape[-1:], p["rnn.norm.weight"], p["rnn.norm.bias"], 1e-5)
     return feat, h1
 
 
-def actor_logits(p, obs, h0, avail=None):
+def actor_logits(p, obs, h0, avail=None, taps=None):
     """R_Actor trunk + Categorical head (modules/agents/ippo_actor.py:43-72,
     utils/mappo_utils/distributions.py:64-68): masked logits [R, n_act], h1."""
-    feat, h1 = trunk_forward(p, obs, h0)
+    feat, h1 = trunk_forward(p, obs, h0, taps)
     logits = feat @ p["act.action_out.linear.weight"].t() + p["act.action_out.linear.bias"]
     if avail is not None:
         logits = torch.where(avail == 0, torch.full_like(logits, -1e10), logits)
@@ -272,10 +278,10 @@ def categorical_stats(logits, actions=None):
     return logp_all, lp, ent
 
 
-def critic_value(p, obs, h0):
+def critic_value(p, obs, h0, taps=None):
     """R_Critic.forward (modules/critics/ippo_critic.py:47-65); PopArt is a plain
     Linear here (utils/mappo_utils/popart.py:41-46)."""
-    feat, h1 = trunk_forward(p, obs, h0)
+    feat, h1 = trunk_forward(p, obs, h0, taps)
     v = feat @ p["v_out.weight"].t() + p["v_out.bias"]
     return v.squeeze(-1), h1
 
@@ -329,7 +335,7 @@ def gae_returns(values_all, rewards, alive_all, gamma=0.99, lam=0.95):
     values_all [Bf,T+1], rewards [Bf,T], alive_all [Bf,T+1] -> returns [Bf,T]."""
     T = rewards.shape[1]
     ret = torch.empty_like(rewards)
-    gae = torch.zeros(rewards.shape[0])
+    gae = torch.zeros(rewards.shape[0], dtype=rewards.dtype, device=rewards.device)
     for t in reversed(range(T)):
         delta = rewards[:, t] + gamma * values_all[:, t + 1] * alive_all[:, t + 1] - values_all[:, t]
         gae = delta + gamma * lam * alive_all[:, t + 1] * gae
@@ -396,13 +402,23 @@ class AdamState:
 
     def step(self, grads):
         self.t += 1
-        bc1 = 1 - self.b1 ** self.t
-        bc2 = 1 - self.b2 ** self.t
-        for p, g, m, v in zip(self.params, grads, self.m, self.v):
-            m.mul_(self.b1).add_(g, alpha=1 - self.b1)
-            v.mul_(self.b2).addcmul_(g, g, value=1 - self.b2)
-            denom = (v.sqrt() / math.sqrt(bc2)).add_(self.eps)
-            p.addcdiv_(m, denom, value=-self.lr / bc1)
+        adam_update(self.params, grads, self.m, self.v, self.t, self.lr, self.eps, self.b1, self.b2)
+
+    def clip_step(self, grads, max_norm):
+        """clip_grad_norm_(max_norm) and then ``step``; returns the norm before clipping."""
+        self.t += 1
+        return clip_adam_step(self.params, grads, self.m, self.v, self.t, self.lr, self.eps, max_norm, self.b1, self.b2)
+
+
+def adam_update(params, grads, m, v, step, lr, eps, b1=0.9, b2=0.999):
+    """Adam step number ``step`` (1-based) on lists of tensors, in place: torch.optim.Adam's arithmetic (see AdamState)."""
+    bc1 = 1 - b1 ** step
+    bc2 = 1 - b2 ** step
+    for p_, g, m_, v_ in zip(params, grads, m, v):
+        m_.mul_(b1).add_(g, alpha=1 - b1)
+        v_.mul_(b2).addcmul_(g, g, value=1 - b2)
+        denom = (v_.sqrt() / math.sqrt(bc2)).add_(eps)
+        p_.addcdiv_(m_, denom, value=-lr / bc1)
 
 
 def clip_grads(grads, max_norm):
@@ -411,6 +427,75 @@ def clip_grads(grads, max_norm):
     total = torch.sqrt(sum((g.detach() ** 2).sum() for g in grads))
     coef = torch.clamp(max_norm / (total + 1e-6), max=1.0)
     return [g * coef for g in grads], total
+
+
+def clip_adam_step(params, grads, m, v, step, lr, eps, max_norm, b1=0.9, b2=0.999):
+    """One optimiser step of the IPPO update (learners/ippo_learner.py:205-221): clip_grad_norm_(max_norm) of the raw
+    gradients, then Adam step ``step``; params / m / v are updated in place, in their own dtype.  Returns the norm
+    before clipping."""
+    clipped, total = clip_grads(grads, max_norm)
+    adam_update(params, clipped, m, v, step, lr, eps, b1, b2)
+    return total
+
+
+def ppo_epoch(actor_p, critic_p, flat, args, idx=None, rows_out=False):
+    """One PPO epoch of IPPOLearner.train (learners/ippo_learner.py:181-221) at fixed weights, up to the raw gradients.
+
+    ``flat`` holds the per-row tensors of the trained episodes (obs, rnn_a, rnn_c, act, avail, and the pre-update ret,
+    alive, old_lp, adv (normalised), old_v); ``idx`` is the epoch's row order (None: as stored).  Returns a dict: the
+    raw gradients ``grads_actor`` / ``grads_critic`` (keyed like ACTOR_TRAINABLE / CRITIC_TRAINABLE), the 0-d tensors
+    ``policy_loss``, ``value_loss``, ``dist_entropy``, ``ratio`` (mean), ``actor_grad_norm``, ``critic_grad_norm``.
+    ``rows_out`` adds, per row in that order: ``logp``, ``value``, ``entropy``, ``ratio_rows``, the value errors
+    ``e_orig`` = ret - v and ``e_clip`` = ret - v_clipped with their losses ``l_orig`` / ``l_clip``; the branch flags
+    ``ratio_clipped`` (the clipped surrogate is the minimum: no policy gradient), ``value_clip_chosen`` (the clipped
+    value loss is the maximum), ``huber_outer`` (|e| > delta for the chosen e) and ``huber_dead`` (e < -delta: no
+    gradient); the GRU inputs ``a2_actor`` / ``a2_critic`` and the loss gradients w.r.t. their projections
+    ``d_gi_actor`` / ``d_gi_critic``; the two ReLUs' inputs ``z_actor`` / ``z_critic`` (z1, z2) and the loss gradients
+    w.r.t. their outputs ``d_relu_actor`` / ``d_relu_critic``."""
+    mb = flat if idx is None else {k: v[idx] for k, v in flat.items()}
+    a_tr = [actor_p[k] for k in ACTOR_TRAINABLE]
+    c_tr = [critic_p[k] for k in CRITIC_TRAINABLE]
+    fresh = [t for t in a_tr + c_tr if not t.requires_grad]
+    for t in fresh:
+        t.requires_grad_(True)
+    tap_a, tap_c = ({}, {}) if rows_out else (None, None)
+    try:
+        with torch.enable_grad():
+            logits, _ = actor_logits(actor_p, mb["obs"], mb["rnn_a"], mb["avail"], taps=tap_a)
+            _, lp, ent = categorical_stats(logits, mb["act"])
+            ent_mean = ent.mean()                                                    # act.py:164 (unmasked)
+            values, _ = critic_value(critic_p, mb["obs"], mb["rnn_c"], taps=tap_c)
+            pol_loss, ratio = policy_loss_terms(lp, mb["old_lp"], mb["adv"], mb["alive"], args.clip_param)
+            extra_a = [tap_a["gi"], tap_a["r1"], tap_a["r2"]] if rows_out else []
+            g_a = torch.autograd.grad(pol_loss - ent_mean * args.entropy_coef, a_tr + extra_a)
+            v_loss = value_loss_terms(values, mb["old_v"], mb["ret"], mb["alive"], args.clip_param, args.huber_delta)
+            extra_c = [tap_c["gi"], tap_c["r1"], tap_c["r2"]] if rows_out else []
+            g_c = torch.autograd.grad(v_loss * args.value_loss_coef, c_tr + extra_c)
+    finally:
+        for t in fresh:
+            t.requires_grad_(False)
+    raw_a, raw_c = list(g_a[:len(a_tr)]), list(g_c[:len(c_tr)])
+    norm = lambda gs: torch.sqrt(sum((g.detach() ** 2).sum() for g in gs))         # clip_grads' total
+    out = dict(grads_actor=dict(zip(ACTOR_TRAINABLE, raw_a)), grads_critic=dict(zip(CRITIC_TRAINABLE, raw_c)),
+               policy_loss=pol_loss.detach(), value_loss=v_loss.detach(), dist_entropy=ent_mean.detach(),
+               ratio=ratio.mean().detach(), actor_grad_norm=norm(raw_a), critic_grad_norm=norm(raw_c))
+    if rows_out:
+        with torch.no_grad():
+            clip, d = args.clip_param, args.huber_delta
+            v = values.detach()
+            v_clip = mb["old_v"] + (v - mb["old_v"]).clamp(-clip, clip)
+            e_orig, e_clip = mb["ret"] - v, mb["ret"] - v_clip
+            l_orig, l_clip = huber_one_sided(e_orig, d), huber_one_sided(e_clip, d)
+            r = ratio.detach()
+            chosen = l_clip > l_orig
+            e = torch.where(chosen, e_clip, e_orig)
+            out.update(logp=lp.detach(), value=v, entropy=ent.detach(), ratio_rows=r, e_orig=e_orig, e_clip=e_clip,
+                       l_orig=l_orig, l_clip=l_clip, ratio_clipped=r.clamp(1 - clip, 1 + clip) * mb["adv"] < r * mb["adv"],
+                       value_clip_chosen=chosen, huber_outer=e.abs() > d, huber_dead=e < -d,
+                       a2_actor=tap_a["a2"].detach(), a2_critic=tap_c["a2"].detach(), d_gi_actor=g_a[-3], d_gi_critic=g_c[-3],
+                       z_actor=(tap_a["z1"].detach(), tap_a["z2"].detach()), z_critic=(tap_c["z1"].detach(), tap_c["z2"].detach()),
+                       d_relu_actor=tuple(g_a[-2:]), d_relu_critic=tuple(g_c[-2:]))
+    return out
 
 
 def train_agent(actor_p, critic_p, batch, agent_id, args, opt_a=None, opt_c=None,
@@ -465,28 +550,15 @@ def train_agent(actor_p, critic_p, batch, agent_id, args, opt_a=None, opt_c=None
         # batch_size*T rows; available_actions loses its LAST EPISODE (:394) which is
         # consistent with indices < batch_size*T when batch_size <= Bf - 1.
         idx = perms[ep] if perms is not None else torch.randperm(rows)
-        mb = {k: v[idx] for k, v in flat.items()}
-        logits, _ = actor_logits(actor_p, mb["obs"], mb["rnn_a"], mb["avail"])
-        _, lp, ent = categorical_stats(logits, mb["act"])
-        ent_mean = ent.mean()                                                    # act.py:164 (unmasked)
-        values, _ = critic_value(critic_p, mb["obs"], mb["rnn_c"])
-        pol_loss, ratio = policy_loss_terms(lp, mb["old_lp"], mb["adv"], mb["alive"], args.clip_param)
-        g_a = torch.autograd.grad(pol_loss - ent_mean * args.entropy_coef, a_tr)
-        raw_a = [g.clone() for g in g_a]
-        g_a, n_a = clip_grads(g_a, args.max_grad_norm)
-        v_loss = value_loss_terms(values, mb["old_v"], mb["ret"], mb["alive"],
-                                  args.clip_param, args.huber_delta)
-        g_c = torch.autograd.grad(v_loss * args.value_loss_coef, c_tr)
-        raw_c = [g.clone() for g in g_c]
-        g_c, n_c = clip_grads(g_c, args.max_grad_norm)
+        e = ppo_epoch(actor_p, critic_p, flat, args, idx)
         with torch.no_grad():
-            opt_a.step(g_a)
-            opt_c.step(g_c)
-        stats.append(dict(value_loss=v_loss.item(), policy_loss=pol_loss.item(),
-                          dist_entropy=ent_mean.item(), actor_grad_norm=n_a.item(),
-                          critic_grad_norm=n_c.item(), ratio=ratio.mean().item(),
-                          grads_actor=dict(zip(ACTOR_TRAINABLE, raw_a)) if ep == 0 else None,
-                          grads_critic=dict(zip(CRITIC_TRAINABLE, raw_c)) if ep == 0 else None))
+            n_a = opt_a.clip_step([e["grads_actor"][k] for k in ACTOR_TRAINABLE], args.max_grad_norm)
+            n_c = opt_c.clip_step([e["grads_critic"][k] for k in CRITIC_TRAINABLE], args.max_grad_norm)
+        stats.append(dict(value_loss=e["value_loss"].item(), policy_loss=e["policy_loss"].item(),
+                          dist_entropy=e["dist_entropy"].item(), actor_grad_norm=n_a.item(),
+                          critic_grad_norm=n_c.item(), ratio=e["ratio"].item(),
+                          grads_actor=e["grads_actor"] if ep == 0 else None,
+                          grads_critic=e["grads_critic"] if ep == 0 else None))
     for t in a_tr + c_tr:
         t.requires_grad_(False)
     pre = dict(values_all=v_all, returns=returns, advantages=adv, old_logp=old_lp.view(Bf, T))

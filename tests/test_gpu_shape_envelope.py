@@ -269,28 +269,19 @@ def test_k1c_scalar_staging_path_for_an_unaligned_row_pitch():
 
 
 # ---- IPPO learner at 6 and 8 actions -----------------------------------------------------------------------------------
-@pytest.mark.parametrize("nA", [6, 8])
-def test_learner_six_and_eight_actions_vs_oracle(nA):
-    """IPPOLearner.train at the 7-slot MPE width (3 agents, 3 landmarks, 1 random agent: feat_dim 308 + nA + 3, not a
-    multiple of 32) with nA actions, many rows masking actions other than the one taken: first-epoch gradients of agent 1
-    against O.train_agent, post-update weights with the bounds of test_learner_vs_oracle_baseline_shape."""
-    _need_gpu()
-    import importlib.util
-    spec = importlib.util.spec_from_file_location("test_gpu_learner", os.path.join(ROOT, "tests", "test_gpu_learner.py"))
-    tgl = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(tgl)
+def masked_mpe_learner_case(nA, B, T, seed, **overrides):
+    """Learner inputs at the 7-slot MPE width (3 agents, 3 landmarks, 1 random agent: feat_dim 308 + nA + 3, not a
+    multiple of 32) with nA actions: B episodes of T steps, random availability masks (the action taken is always
+    available), terminations of 3 % per step, a x30 policy head.  Returns (args, data, actors, critics, feat_dim)."""
     from iplan_b200.config import controller_input_dim, make_args
     from iplan_b200.modules.flat import ParamStack
-    from oracle import iplan_oracle as O
-    _nt()
-    B, T = 12, 20
     args = make_args("MPE", num_random_agents=1, n_actions=nA, episode_limit=T, batch_size_run=B, buffer_size=B,
-                     batch_size=B - 1, use_cuda=True, device="cuda")
+                     batch_size=B - 1, use_cuda=True, device="cuda", **overrides)
     A, N, o, L, D, R = args.n_agents, args.max_vehicle_num, args.obs_shape_single, args.latent_dim, args.attention_dim, args.rnn_hidden_dim
     assert N == 7
     F = controller_input_dim(args)
     assert F == 308 + nA + A and F % 32 != 0
-    rng = np.random.default_rng(nA)
+    rng = np.random.default_rng(seed)
     hist = rng.uniform(-1, 1, size=(B, T + 1, A, N, o)).astype(np.float32)
     acts = rng.integers(0, nA, size=(B, T + 1, A, 1))
     avail = (rng.uniform(size=(B, T + 1, A, nA)) < 0.5).astype(np.int64)
@@ -302,13 +293,30 @@ def test_learner_six_and_eight_actions_vs_oracle(nA):
                 rnn_states_critics=rng.uniform(-1, 1, size=(B, T + 1, A, R)).astype(np.float32),
                 actions=acts, avail_actions=avail, reward=(rng.normal(size=(B, T + 1, A, 1)) * 2).astype(np.float32),
                 terminated=term)
-    torch.manual_seed(nA)
+    torch.manual_seed(seed)
     a0, c0 = ParamStack("actor", A, (F, nA)), ParamStack("critic", A, (F,))
     with torch.no_grad():
         for n in a0.nets:
             n.act.action_out.linear.weight.mul_(30.0)
     actors = [{k: v.clone() for k, v in n.state_dict().items()} for n in a0.nets]
     critics = [{k: v.clone() for k, v in n.state_dict().items()} for n in c0.nets]
+    return args, data, actors, critics, F
+
+
+@pytest.mark.parametrize("nA", [6, 8])
+def test_learner_six_and_eight_actions_vs_oracle(nA):
+    """IPPOLearner.train at the 7-slot MPE width (3 agents, 3 landmarks, 1 random agent: feat_dim 308 + nA + 3, not a
+    multiple of 32) with nA actions, many rows masking actions other than the one taken: first-epoch gradients of agent 1
+    against O.train_agent, post-update weights with the bounds of test_learner_vs_oracle_baseline_shape."""
+    _need_gpu()
+    import importlib.util
+    spec = importlib.util.spec_from_file_location("test_gpu_learner", os.path.join(ROOT, "tests", "test_gpu_learner.py"))
+    tgl = importlib.util.module_from_spec(spec)
+    spec.loader.exec_module(tgl)
+    from oracle import iplan_oracle as O
+    _nt()
+    B, T = 12, 20
+    args, data, actors, critics, F = masked_mpe_learner_case(nA, B, T, seed=nA)
     batch, mac, learner, _ = tgl.build(args, data, actors, critics)
     learner.keep_pre = True
     learner.insert_episode_batch(batch)
