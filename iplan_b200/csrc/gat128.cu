@@ -23,6 +23,7 @@
 // torch.matmul, iplan_b200/nova/gat128.py); this file holds the recurrence, the attention and the GRUCell gate kernels.
 #include "common.cuh"
 #include "gat_common.cuh"
+#include "hopper.cuh"
 
 namespace iplan {
 
@@ -44,28 +45,12 @@ struct Gat128Args {
     int n_agents; int64_t n_items; int items_per_cta;
 };
 
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void sts16(uint32_t addr, uint16_t v) {
     asm volatile("st.shared.u16 [%0], %1;" ::"r"(addr), "h"(v) : "memory");
 }
 __device__ __forceinline__ void sts128(uint32_t addr, uint32_t x, uint32_t y, uint32_t z, uint32_t w) {
     asm volatile("st.shared.v4.u32 [%0], {%1,%2,%3,%4};" ::"r"(addr), "r"(x), "r"(y), "r"(z), "r"(w) : "memory");
 }
-// generic-proxy writes to shared memory -> visible to the async proxy (wgmma operand reads)
-__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-// Byte offset of 16-byte chunk `chunk` (0..7) of row `row` in a K-major SWIZZLE_128B tile (rows of 128 B, base 1024-aligned)
-__device__ __forceinline__ uint32_t swz128(int row, int chunk) {
-    return (uint32_t)(row >> 3) * 1024u + (uint32_t)(row & 7) * 128u + (uint32_t)((chunk ^ (row & 7)) << 4);
-}
-// wgmma shared-memory matrix descriptor of a K-major SWIZZLE_128B tile: rows of 128 B, 8-row groups 1024 B apart (stride
-// byte offset); the leading byte offset is unused when K fits one swizzle atom.  A k-block of 16 f16 starts 32 B further.
-__device__ __forceinline__ uint64_t wgmma_desc(uint32_t smem_addr) {
-    return (uint64_t)((smem_addr & 0x3FFFF) >> 4) | ((uint64_t)1 << 16) | ((uint64_t)(1024 >> 4) << 32) | ((uint64_t)1 << 62);
-}
-__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
-template <int N_PENDING>
-__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N_PENDING) : "memory"); }
 // D[64 x 16] += A[64 x 16] . B[16 x 16]^T, both operands K-major in shared memory, f16 in, fp32 accumulate
 // accumulate == 0: D = A . B^T (the old contents of d are ignored)
 __device__ __forceinline__ void wgmma_m64n16k16(float (&d)[8], uint64_t da, uint64_t db, int accumulate) {

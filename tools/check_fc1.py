@@ -3,6 +3,10 @@
 (iplan_learner_fc1_backward: G = dZ1^T X and the fc1.weight / feature_norm gradients).
 
     python tools/check_fc1.py            # a ragged small case, one agent at full width, the bench shape
+
+At the bench shape it also times the two product kernels alone (torch.profiler, several launches) and prints the rate of
+the X stream (Xh + Xl, 4 bytes per element, read once per product) against the H100 SXM's 3.35 TB/s of HBM3, and the
+rate of the tensor work (three f16 products per fp32 product).
 """
 import os
 import sys
@@ -14,7 +18,32 @@ from iplan_b200 import _lib                          # noqa: E402
 from iplan_b200.modules.flat import ParamStack       # noqa: E402
 
 
-def run(A, rows, F, n_act=5, reps=5):
+HBM_TBS = 3.35                                       # H100 SXM data sheet
+
+
+def kernel_ms(call, name, reps):
+    """Mean device time of the kernels whose name contains `name`, over `reps` calls."""
+    from torch.profiler import ProfilerActivity, profile
+    call()
+    torch.cuda.synchronize()
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        for _ in range(reps):
+            call()
+        torch.cuda.synchronize()
+    us = sum(getattr(e, "device_time_total", 0) or getattr(e, "cuda_time_total", 0)
+             for e in prof.key_averages() if name in e.key)
+    return us / 1e3 / reps
+
+
+def rates(what, ms, A, rows, Fp):
+    x_bytes = A * rows * Fp * 4                      # Xh + Xl
+    flops = 3 * 2 * A * rows * 128 * Fp              # hi*hi + lo*hi + hi*lo
+    gbs = x_bytes / ms / 1e6
+    print(f"  {what} kernel: {ms:.3f} ms; X stream {gbs:.0f} GB/s = {gbs / (HBM_TBS * 1e3):.0%} of {HBM_TBS} TB/s; "
+          f"tensor work {flops / ms / 1e9:.0f} TFLOP/s", flush=True)
+
+
+def run(A, rows, F, n_act=5, reps=5, kernel_rates=False):
     """Largest error relative to the fp64 result's magnitude, over the forward Z1 and the backward G."""
     torch.manual_seed(0)
     dev = "cuda"
@@ -45,9 +74,10 @@ def run(A, rows, F, n_act=5, reps=5):
         return e0.elapsed_time(e1) / reps
 
     Z = torch.full((A, rows, 128), float("nan"), device=dev)
-    t_fwd = timed(lambda: _lib.check(lib.iplan_learner_fc1_forward(
+    fwd = lambda: _lib.check(lib.iplan_learner_fc1_forward(
         P(actor.flat), actor.stride(), P(critic.flat), critic.stride(), P(Xh), P(Xl), Xh.stride(0), Fp, F, rows, A, P(stat),
-        P(Wh), P(Wl), P(ws), P(cc), P(Z), st), "fc1_forward"))
+        P(Wh), P(Wl), P(ws), P(cc), P(Z), st), "fc1_forward")
+    t_fwd = timed(fwd)
     xs = X[..., :F].double()
     mu, var = xs.mean(-1, keepdim=True), xs.var(-1, unbiased=False, keepdim=True)
     xn = (xs - mu) / torch.sqrt(var + 1e-5)
@@ -63,19 +93,24 @@ def run(A, rows, F, n_act=5, reps=5):
     SM = torch.randn(A, 2, 128, device=dev) * 1e-3
     Dh, Dl, gs, G = hz(A, rows, 128), hz(A, rows, 128), z(2 * A), z(A, 128, Fp)
     ga, gc = torch.zeros_like(actor.flat), torch.zeros_like(critic.flat)
-    t_bwd = timed(lambda: _lib.check(lib.iplan_learner_fc1_backward(
+    bwd = lambda: _lib.check(lib.iplan_learner_fc1_backward(
         P(actor.flat), actor.stride(), P(critic.flat), critic.stride(), P(ga), P(gc), P(Xh), P(Xl), Xh.stride(0), Fp, F, rows, A,
-        P(dZ), P(Dh), P(Dl), P(gs), P(SM), P(G), st), "fc1_backward"))
+        P(dZ), P(Dh), P(Dl), P(gs), P(SM), P(G), st), "fc1_backward")
+    t_bwd = timed(bwd)
     Gref = torch.einsum("ark,arf->akf", dZ.double(), X.double())
     d_bwd = (G.double() - Gref).abs().max().item() / Gref.abs().max().item()
     print(f"A={A} rows={rows} F={F}: forward {t_fwd:.3f} ms, max rel|Z1 - fp64| = {d_fwd:.3e}; "
           f"backward (all launches) {t_bwd:.3f} ms, max rel|G - fp64| = {d_bwd:.3e}; "
           f"nan: {bool(torch.isnan(Z).any() or torch.isnan(G).any())}", flush=True)
+    if kernel_rates:
+        print(f"  {torch.cuda.get_device_name()}:")
+        rates("forward (fc1_fwd_wgmma_kernel)", kernel_ms(fwd, "fc1_fwd_wgmma_kernel", 10), A, rows, Fp)
+        rates("backward (fc1_bwd_wgmma_kernel)", kernel_ms(bwd, "fc1_bwd_wgmma_kernel", 10), A, rows, Fp)
     return max(d_fwd, d_bwd)
 
 
 if __name__ == "__main__":
     ok = run(2, 300, 272) < 1e-5            # MPE width: ragged k (Fp = 288) and ragged rows
     ok &= run(1, 128, 2485) < 1e-5
-    ok &= run(5, 46592, 2485, reps=3) < 1e-5   # bench shape: 512 envs x 91 steps
+    ok &= run(5, 46592, 2485, reps=3, kernel_rates=True) < 1e-5   # bench shape: 512 envs x 91 steps
     print("OK" if ok else "MISMATCH")
