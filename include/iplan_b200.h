@@ -351,6 +351,10 @@ typedef struct {
     float grad_scale;              /* power-of-two loss scale: every gradient buffer holds grad_scale * g
                                       (keeps the backward operands inside f16's normal range for the
                                       split-f16 tensor-core products); pass the same value to iplan_learner_adam */
+    const int32_t* train_rows;     /* NULL: rows are the packed episodes, row (b,t) trains iff t < T1-1 and b < n_train_eps.
+                                      Else [A]: the rows are a gathered mini-batch (iplan_learner_gather_rows) and agent
+                                      a's rows 0 .. train_rows[a]-1 train, whatever T1 / n_train_eps say; `norm` then
+                                      carries the mini-batch's own 1/sum(alive) and 1/rows */
 } iplan_learner_ctx;
 
 /* Z1 -> LN/ReLU -> fc2 -> LN/ReLU -> GRU step -> LN -> heads (R_Actor.evaluate_actions,
@@ -360,6 +364,23 @@ typedef struct {
  *   entropy bonus) with their backward; leaves dZ1*rstd in Z1 and every gradient except
  *   fc1.weight / feature_norm in g_actor / g_critic. */
 int iplan_learner_tail(const iplan_learner_ctx* ctx, int train, void* stream);
+
+/* One shuffled mini-batch (generate_data :368-424) as dense rows: destination row j of agent a is source row
+ * idx[a][j] of the packed store (idx < 0: padding, a copy of source row 0 that must lie past train_rows[a]).
+ * Every array is [A][rows] rows of its width, source with rows_src rows per agent, destination with rows_dst.
+ * The fc1 products and the tail then run on the destination unchanged, with rows = rows_dst. */
+typedef struct {
+    const int32_t* idx;            /* [A][rows_dst] */
+    int64_t rows_src, rows_dst;
+    int n_agents, ldx, n_actions;  /* ldx % 8 == 0 (16-byte vectors of __half) */
+    const void* Xh; const void* Xl; void* Xh_out; void* Xl_out;              /* __half [ldx] */
+    const float* stat; float* stat_out;                                     /* [2] */
+    const float* rnn_a; const float* rnn_c; float* rnn_a_out; float* rnn_c_out;   /* [64] */
+    const int32_t* actions; int32_t* actions_out;
+    const uint8_t* avail; uint8_t* avail_out;                               /* [n_actions] */
+    const float* scalars[5]; float* scalars_out[5];   /* old_logp, old_value, returns, adv_raw, alive */
+} iplan_gather_args;
+int iplan_learner_gather_rows(const iplan_gather_args* args, void* stream);
 
 /* fc1.weight and feature_norm gradients from dZ1 (left in Z1 by the train tail): tensor-core
  * product G = dZ1^T X over the f16 copies.  Scratch: Dh/Dl [A][rows][128] __half (scaled split of

@@ -73,6 +73,7 @@ _SIGNATURES = {
     "iplan_learner_x_split": (_i, [_p, _i64, _p, _p, _p]),
     "iplan_learner_fc1_forward": (_i, [_p, _i64, _p, _i64, _p, _p, _i64, _i, _i, _i64, _i, _p, _p, _p, _p, _p, _p, _p]),
     "iplan_learner_tail": (_i, [_p, _i, _p]),
+    "iplan_learner_gather_rows": (_i, [_p, _p]),
     "iplan_learner_fc1_backward": (_i, [_p, _i64, _p, _i64, _p, _p, _p, _p, _i64, _i, _i, _i64, _i,
                                         _p, _p, _p, _p, _p, _p, _p]),
     "iplan_learner_gae": (_i, [_p, _p, _p, _f, _f, _i, _i, _i, _i, _p, _p, _p, _p]),
@@ -93,7 +94,17 @@ class LearnerCtx(C.Structure):
                 ("logp_out", _p), ("ent_out", _p), ("value_out", _p),
                 ("old_logp", _p), ("old_value", _p), ("returns", _p), ("adv_raw", _p), ("alive", _p),
                 ("norm", _p), ("stats", _p),
-                ("clip", _f), ("ent_coef", _f), ("v_coef", _f), ("huber_delta", _f), ("grad_scale", _f)]
+                ("clip", _f), ("ent_coef", _f), ("v_coef", _f), ("huber_delta", _f), ("grad_scale", _f),
+                ("train_rows", _p)]
+
+
+class GatherArgs(C.Structure):
+    """iplan_gather_args (include/iplan_b200.h)."""
+    _fields_ = [("idx", _p), ("rows_src", _i64), ("rows_dst", _i64), ("n_agents", _i), ("ldx", _i), ("n_actions", _i),
+                ("Xh", _p), ("Xl", _p), ("Xh_out", _p), ("Xl_out", _p), ("stat", _p), ("stat_out", _p),
+                ("rnn_a", _p), ("rnn_c", _p), ("rnn_a_out", _p), ("rnn_c_out", _p),
+                ("actions", _p), ("actions_out", _p), ("avail", _p), ("avail_out", _p),
+                ("scalars", _p * 5), ("scalars_out", _p * 5)]
 
 
 def _bind(signatures):

@@ -6,7 +6,8 @@
 // input of episode b at time t (EpisodeBatch packed layout).  "net" = 2*a + {0 actor, 1 critic}.
 //
 // Per PPO epoch (reference :284-310; num_mini_batch = 1 so a minibatch is every training
-// row in permuted order — the permutation only reorders sums):
+// row in permuted order — the permutation only reorders sums; with more mini-batches gather_rows copies each one's
+// rows into dense buffers and the same kernels run on those, once per mini-batch):
 //   fc1_prep        fold LayerNorm(F) into fc1:  W' = gamma.W1, ws = sum_f W', c = W1.beta + b1
 //   fc1_fwd         Z1 = rstd_r (X W'^T - mu_r ws) + c                      (both nets, N=128)
 //   ln_relu_fwd     A1 = LN(ReLU(Z1));  linear_fwd Z2 = A1 W2^T + b2;  A2 = LN(ReLU(Z2))
@@ -207,6 +208,7 @@ struct HeadArgs {
     float clip, ent_coef, v_coef, huber_delta;
     float gscale;                  // power-of-two loss scale applied to d loss / d logits|value (undone in adam)
     float* stats;                 // [A][8]: sums of policy-loss, value-loss, entropy, ratio (already normalised)
+    const int32_t* train_rows;    // NULL, or [A]: the rows are a gathered mini-batch whose first train_rows[a] rows train
     int train;
 };
 
@@ -324,7 +326,7 @@ __global__ void __launch_bounds__(HEAD_THREADS, 3) gru_head_kernel(HeadArgs h) {
         }
 
         const int64_t ridx = (int64_t)a * h.rows + r;
-        const bool train_row = valid && h.train && t < h.T1 - 1 && b < h.n_train_eps;
+        const bool train_row = valid && h.train && (h.train_rows ? r < h.train_rows[a] : t < h.T1 - 1 && b < h.n_train_eps);
         float dA[HU];                         // gradient wrt the LN3 output
 #pragma unroll
         for (int u = 0; u < HU; ++u) dA[u] = 0.0f;
@@ -608,6 +610,36 @@ __global__ void adam_kernel(float* __restrict__ p, const float* __restrict__ g, 
     }
 }
 
+// ---------------------------------------------------------------------------------------
+// gather_rows: one shuffled mini-batch as dense rows, so that the TMA / wgmma fc1 kernels (which load tiles, not row
+// lists) and the tail run on it as they run on the packed store.  One warp per destination row: the two f16 operand rows
+// as 16-byte vectors, the two stored hidden rows, and the row's scalars.
+// ---------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(256) gather_rows_kernel(iplan_gather_args g) {
+    const int a = blockIdx.y, lane = threadIdx.x & 31;
+    const int64_t warps = (int64_t)gridDim.x * (blockDim.x >> 5);
+    const int vec = g.ldx / 8;                                               // uint4 = 8 halves
+    for (int64_t j = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); j < g.rows_dst; j += warps) {
+        const int64_t d = (int64_t)a * g.rows_dst + j;
+        const int32_t i = g.idx[d];
+        const int64_t s = (int64_t)a * g.rows_src + (i < 0 ? 0 : i);
+        const uint4* xh = reinterpret_cast<const uint4*>(static_cast<const __half*>(g.Xh) + s * g.ldx);
+        const uint4* xl = reinterpret_cast<const uint4*>(static_cast<const __half*>(g.Xl) + s * g.ldx);
+        uint4* oh = reinterpret_cast<uint4*>(static_cast<__half*>(g.Xh_out) + d * g.ldx);
+        uint4* ol = reinterpret_cast<uint4*>(static_cast<__half*>(g.Xl_out) + d * g.ldx);
+        for (int v = lane; v < vec; v += 32) { oh[v] = __ldg(xh + v); ol[v] = __ldg(xl + v); }
+        if (lane < RH / 4) {
+            reinterpret_cast<float4*>(g.rnn_a_out + d * RH)[lane] = __ldg(reinterpret_cast<const float4*>(g.rnn_a + s * RH) + lane);
+        } else {
+            reinterpret_cast<float4*>(g.rnn_c_out + d * RH)[lane - RH / 4] = __ldg(reinterpret_cast<const float4*>(g.rnn_c + s * RH) + lane - RH / 4);
+        }
+        if (lane < 5) g.scalars_out[lane][d] = g.scalars[lane][s];
+        else if (lane < 7) g.stat_out[d * 2 + lane - 5] = g.stat[s * 2 + lane - 5];
+        else if (lane == 7) g.actions_out[d] = g.actions[s];
+        else if (lane - 8 < g.n_actions) g.avail_out[d * g.n_actions + lane - 8] = g.avail[s * g.n_actions + lane - 8];
+    }
+}
+
 }  // namespace iplan
 
 // =======================================================================================
@@ -662,7 +694,7 @@ extern "C" int iplan_learner_tail(const iplan_learner_ctx* c, int train, void* s
     h.old_logp = c->old_logp; h.old_value = c->old_value; h.returns = c->returns; h.adv_raw = c->adv_raw; h.alive = c->alive;
     h.norm = c->norm; h.clip = c->clip; h.ent_coef = c->ent_coef; h.v_coef = c->v_coef; h.huber_delta = c->huber_delta;
     h.gscale = c->grad_scale > 0.0f ? c->grad_scale : 1.0f;
-    h.stats = c->stats; h.train = train;
+    h.stats = c->stats; h.train_rows = c->train_rows; h.train = train;
     if (train) IPLAN_REQUIRE(c->g_actor && c->g_critic && c->old_logp && c->old_value && c->returns && c->adv_raw && c->alive && c->norm && c->stats && c->SM && c->stat,
                              "learner_tail: train mode needs gradient/loss buffers");
     static int tail_impl = -1;          // 0 = fused kernel (default), 1 = the twelve separate kernels (cross-check); IPLAN_TAIL_IMPL
@@ -748,6 +780,20 @@ extern "C" int iplan_learner_tail(const iplan_learner_ctx* c, int train, void* s
     }
     count_launch(launches);
     return check_launch("learner_tail");
+}
+
+extern "C" int iplan_learner_gather_rows(const iplan_gather_args* g, void* stream) {
+    IPLAN_REQUIRE(g && g->idx && g->Xh && g->Xl && g->Xh_out && g->Xl_out && g->stat && g->stat_out && g->rnn_a && g->rnn_c &&
+                  g->rnn_a_out && g->rnn_c_out && g->actions && g->actions_out && g->avail && g->avail_out, "gather_rows: null array");
+    for (int i = 0; i < 5; ++i) IPLAN_REQUIRE(g->scalars[i] && g->scalars_out[i], "gather_rows: null scalar array %d", i);
+    IPLAN_REQUIRE(g->rows_src > 0 && g->rows_dst > 0 && g->n_agents > 0 && g->ldx > 0 && g->ldx % 8 == 0 &&
+                  g->n_actions > 0 && g->n_actions <= IPLAN_MAX_ACT, "gather_rows: bad sizes");
+    IPLAN_REQUIRE((((uintptr_t)g->Xh | (uintptr_t)g->Xl | (uintptr_t)g->Xh_out | (uintptr_t)g->Xl_out | (uintptr_t)g->rnn_a |
+                    (uintptr_t)g->rnn_c | (uintptr_t)g->rnn_a_out | (uintptr_t)g->rnn_c_out) & 15) == 0, "gather_rows: rows need 16-byte alignment");
+    dim3 grid((unsigned)std::min<int64_t>((g->rows_dst + 7) / 8, sm_count() * 8), g->n_agents);
+    gather_rows_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(*g);
+    count_launch();
+    return check_launch("gather_rows");
 }
 
 namespace iplan {

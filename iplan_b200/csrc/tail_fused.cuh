@@ -242,6 +242,7 @@ __global__ void __launch_bounds__(TF_THREADS, 1) tail_fused_kernel(TfArgs A) {
     __syncthreads();
 
     const float nrm_mean = h.norm[a * 4], nrm_istd = h.norm[a * 4 + 1], inv_msum = h.norm[a * 4 + 2], inv_rows = h.norm[a * 4 + 3];
+    const int n_tr = h.train_rows ? h.train_rows[a] : -1;                  // gathered mini-batch: its first n_tr rows train
     const int64_t rows = A.rows;
     const int64_t n_tiles = (rows + 15) / 16;
     const float* h0base = (type == 0 ? h.h0a : h.h0c) + a * h.h0_sa;
@@ -407,7 +408,7 @@ __global__ void __launch_bounds__(TF_THREADS, 1) tail_fused_kernel(TfArgs A) {
 #pragma unroll
             for (int l = 0; l < NOUT; ++l) dl[l] = 0.0f;
             const int b = (int)(r / h.T1), tt = (int)(r - (int64_t)b * h.T1);
-            const bool train_row = live && tt < h.T1 - 1 && b < h.n_train_eps;
+            const bool train_row = live && (n_tr >= 0 ? r < n_tr : tt < h.T1 - 1 && b < h.n_train_eps);
             const int64_t ridx = (int64_t)a * h.rows + r;
             if (type == 0) {
                 const int nA = h.n_actions;

@@ -9,6 +9,9 @@ Same constructor ``IPPOLearner(mac, scheme, logger, args)`` and public methods
 (``insert_episode_batch``, ``train``, ``cuda``, ``save_models``, ``load_models``,
 ``lr_decay``, ``compute_returns``); logs the same six statistics under the same keys.
 
+``args.num_mini_batch`` > 1 trains every epoch in that many shuffled sets of rows, one Adam step of each net per set
+(reference generate_data :368-424): see ``_train_minibatches``.
+
 Multi-GPU (new capability, SURVEY §8e): environments are sharded across ranks, each
 rank keeps its own episodes; per ``train()`` one all-reduce of the advantage moments and
 mask sums, and per PPO epoch ONE all-reduce (SUM) of the concatenated actor+critic
@@ -103,7 +106,11 @@ class IPPOLearner:
                      "use_policy_active_masks", "use_max_grad_norm", "use_recurrent_policy"):
             if not getattr(args, flag):
                 raise NotImplementedError(f"only the reference's default IPPO setting is built ({flag}=True)")
-        assert args.num_mini_batch == 1 and args.weight_decay == 0
+        assert args.weight_decay == 0
+        self.num_mini_batch = int(args.num_mini_batch)
+        if not 1 <= self.num_mini_batch <= args.batch_size * args.episode_limit:
+            raise ValueError(f"num_mini_batch={args.num_mini_batch} is not in [1, batch_size * episode_limit = "
+                             f"{args.batch_size * args.episode_limit}]")
         self.clip_param, self.ppo_epoch = args.clip_param, args.ppo_epoch
         self.value_loss_coef, self.entropy_coef = args.value_loss_coef, args.entropy_coef
         self.max_grad_norm, self.huber_delta = args.max_grad_norm, args.huber_delta
@@ -133,6 +140,11 @@ class IPPOLearner:
         self.bucket = parallel.GradBucket()
         self.grad_scale = 1.0
         self.use_dist = True        # False: ignore an active process group (single-rank reference runs in tests)
+        # num_mini_batch > 1: the row permutations of generate_data (reference :384), one per (agent, epoch), drawn on
+        # the CPU from this generator: every rank of a sharded run seeds it alike and so draws the same global ones
+        self.perm_gen = th.Generator().manual_seed(int(getattr(args, "seed", 0) or 0))
+        self.debug_perm = None      # int [A][ppo_epoch][batch_size * T]: the next train() uses these instead of drawing
+        self.mb = None              # the gathered mini-batch's buffers (allocated on the first train() with num_mini_batch > 1)
 
     # ------------------------------------------------------------------------------
     def lr_decay(self, episode, episodes):
@@ -240,12 +252,14 @@ class IPPOLearner:
             e.record()
             ev.append((tag, e))
 
-    def _forward(self, w, ctx, X, A, rows, Fp, F, actor, critic, train):
+    def _forward(self, w, ctx, X, A, rows, Fp, F, actor, critic, train, src=None):
+        """fc1 product + tail over the packed store's rows, or over the gathered mini-batch ``src`` (its first ``rows`` rows)."""
         lib, st = _lib.lib, _lib.stream()
         self._mark("fc1_fwd")
+        Xh, Xl, x_sa, stat = (w["Xh"], w["Xl"], w["Xh"].stride(0), w["stat"]) if src is None else (src["Xh"], src["Xl"], rows * Fp, src["stat"])
         _lib.check(lib.iplan_learner_fc1_forward(
             _lib.ptr(actor), self.stacks["actor"].stride(), _lib.ptr(critic), self.stacks["critic"].stride(),
-            _lib.ptr(w["Xh"]), _lib.ptr(w["Xl"]), w["Xh"].stride(0), Fp, F, rows, A, _lib.ptr(w["stat"]),
+            _lib.ptr(Xh), _lib.ptr(Xl), x_sa, Fp, F, rows, A, _lib.ptr(stat),
             _lib.ptr(w["Wh"]), _lib.ptr(w["Wl"]), _lib.ptr(w["ws"]), _lib.ptr(w["cc"]), _lib.ptr(w["Z1"]), st), "fc1_forward")
         import ctypes
         self._mark("tail_train" if train else "tail_eval")
@@ -272,9 +286,9 @@ class IPPOLearner:
         # first batch_size (global) episodes are trained on (generate_data :371-394)
         n_train_global = self.batch_size
         n_train = parallel.shard_train_episodes(rank, world, Bf, n_train_global)
-        # per-row loss gradients are O(1 / sum(alive)) ~ 1 / (rows trained on): scale them by the next
+        # per-row loss gradients are O(1 / sum(alive)) ~ 1 / (rows of one mini-batch): scale them by the next
         # power of two so the split-f16 tensor-core products of the backward see O(1) operands
-        self.grad_scale = float(2 ** max(0, math.ceil(math.log2(max(1, n_train_global * T)))))
+        self.grad_scale = float(2 ** max(0, math.ceil(math.log2(max(1, n_train_global * T // self.num_mini_batch)))))
         w = self._work_buffers(A, rows, Fp)
         actor, critic = self.stacks["actor"].flat, self.stacks["critic"].flat
         X = s["X"]
@@ -307,7 +321,9 @@ class IPPOLearner:
         # ---- PPO epochs ------------------------------------------------------------------
         w["stats"].zero_()
         ga, gc = w["grads"]["actor"], w["grads"]["critic"]
-        for _ in range(self.ppo_epoch):
+        if self.num_mini_batch > 1:
+            self._train_minibatches(w, s, A, Fp, F, n_train, n_train_global, rank, dist, actor, critic)
+        for _ in range(self.ppo_epoch if self.num_mini_batch == 1 else 0):
             ga.zero_(); gc.zero_(); w["SM"].zero_()
             self._forward(w, ctx, X, A, rows, Fp, F, actor, critic, train=True)
             self._mark("fc1_bwd")
@@ -338,7 +354,7 @@ class IPPOLearner:
             part = stats[:, :4].contiguous()
             dist.all_reduce(part)
             stats[:, :4] = part
-        tot = stats.sum(0).cpu() / float(self.ppo_epoch * self.num_mini_batch_ * A)
+        tot = stats.sum(0).cpu() / float(self.ppo_epoch * self.num_mini_batch * A)
         self.train_info = dict(policy_loss=float(tot[0]), value_loss=float(tot[1]), dist_entropy=float(tot[2]),
                                ratio=float(tot[3]), actor_grad_norm=float(tot[4]), critic_grad_norm=float(tot[5]))
         self.count = 0                                      # clear_buffer (:312)
@@ -346,7 +362,130 @@ class IPPOLearner:
             for k in ("value_loss", "policy_loss", "dist_entropy", "actor_grad_norm", "critic_grad_norm", "ratio"):
                 self.logger.log_stat(self.log_prefix + k, self.train_info[k], t_env)
 
-    num_mini_batch_ = 1
+    # ---- num_mini_batch > 1 (reference generate_data :368-424, ppo_update per mini-batch :290-303) ----------------
+    def _draw_perms(self, n):
+        """[A][ppo_epoch][n] int64 on the device: ``debug_perm`` if set (consumed), else drawn agent-major, then epoch
+        (the reference's nesting of generate_data's ``th.randperm``) from the learner's CPU generator."""
+        A, E = self.n_agents, self.ppo_epoch
+        if self.debug_perm is not None:
+            perm, self.debug_perm = th.as_tensor(self.debug_perm), None
+            assert tuple(perm.shape) == (A, E, n), (tuple(perm.shape), (A, E, n))
+        else:
+            perm = th.stack([th.randperm(n, generator=self.perm_gen) for _ in range(A * E)]).view(A, E, n)
+        return perm.to(th.int32).to(self.device).long()
+
+    def _train_minibatches(self, w, s, A, Fp, F, n_train, n_train_global, rank, dist, actor, critic):
+        """The PPO epochs with ``num_mini_batch`` = k > 1: per epoch and agent a permutation of the batch_size * T
+        training rows is cut into k sets of n // k rows (the n % k trailing rows are not trained on in that epoch) and
+        every set takes one clipped Adam step of the actors and one of the critics, its losses normalised over the set.
+        iplan_learner_gather_rows copies a set's rows into dense buffers, on which the fc1 products and the tail run
+        with ``rows`` = the set's size.  Sharded over ranks, a rank gathers the rows of the set it holds (set sizes then
+        differ between agents: the shorter ones are padded with rows that do not train), the denominators are the
+        global ones, and the gradients are all-reduced once per set.
+
+        A set without a single alive row divides by zero in the reference (NaN losses, NaN weights).  Here its policy
+        and value terms are skipped (loss and gradient 0; the entropy bonus, which is not masked, remains) and Adam
+        steps on what is left, as torch.optim.Adam would."""
+        lib, st, P = _lib.lib, _lib.stream(), _lib.ptr
+        k, E, T1, Bf, nA, R = self.num_mini_batch, self.ppo_epoch, self.T1, self.buffer_size, self.n_actions, self.args.rnn_hidden_dim
+        T = T1 - 1
+        n = n_train_global * T
+        mbs = n // k
+        perm = self._draw_perms(n)
+        idx, count = parallel.local_minibatch_rows(perm, k, T, rank * Bf, rank * Bf + n_train)      # [A][E][k][cap], [A][E][k]
+        valid = idx >= 0
+        safe = idx.clamp_min(0)
+        alive_tr = s["alive"][:, :, :T].reshape(A, Bf * T)
+        asum = (alive_tr.gather(1, safe.view(A, -1)).view(idx.shape) * valid).sum(-1).double()       # [A][E][k]
+        if dist:
+            dist.all_reduce(asum)
+        norm_sets = th.empty(E, k, A, 4, device=self.device)
+        norm_sets[..., 0:2] = w["norm"][:, 0:2]
+        norm_sets[..., 2] = th.where(asum > 0, 1.0 / asum, th.zeros_like(asum)).float().permute(1, 2, 0)
+        norm_sets[..., 3] = 1.0 / mbs
+        count_sets = count.permute(1, 2, 0).to(th.int32).contiguous()                                   # [E][k][A]
+        src_rows = th.where(valid, (safe // T) * T1 + safe % T, idx).permute(1, 2, 0, 3).to(th.int32).contiguous()   # [E][k][A][cap]
+        cap = src_rows.shape[-1]
+        rows_set = count_sets.amax(-1).cpu() if dist else th.full((E, k), mbs)
+        cap_alloc = min(mbs, max(1, n_train * T))
+        key = (A, cap_alloc, Fp)
+        if self.mb is None or self.mb["key"] != key:
+            dev = self.device
+            z = lambda *sh, **kw: th.zeros(*sh, device=dev, **kw)
+            self.mb = dict(key=key, Xh=z(A * cap_alloc * Fp, dtype=th.float16), Xl=z(A * cap_alloc * Fp, dtype=th.float16),
+                           stat=z(A * cap_alloc * 2), rnn_a=z(A * cap_alloc * R), rnn_c=z(A * cap_alloc * R),
+                           actions=z(A * cap_alloc, dtype=th.int32), avail=z(A * cap_alloc * nA, dtype=th.uint8),
+                           scalars=[z(A * cap_alloc) for _ in range(5)])
+        mb = self.mb
+        g = _lib.GatherArgs()
+        g.rows_src, g.n_agents, g.ldx, g.n_actions = Bf * T1, A, Fp, nA
+        g.Xh, g.Xl, g.Xh_out, g.Xl_out = P(w["Xh"]), P(w["Xl"]), P(mb["Xh"]), P(mb["Xl"])
+        g.stat, g.stat_out = P(w["stat"]), P(mb["stat"])
+        g.rnn_a, g.rnn_c, g.rnn_a_out, g.rnn_c_out = P(s["rnn_a"]), P(s["rnn_c"]), P(mb["rnn_a"]), P(mb["rnn_c"])
+        g.actions, g.actions_out, g.avail, g.avail_out = P(s["actions"]), P(mb["actions"]), P(s["avail"]), P(mb["avail"])
+        for i, t in enumerate((w["old_logp"], w["old_value"], w["returns"], w["adv"], s["alive"])):
+            g.scalars[i], g.scalars_out[i] = t.data_ptr(), mb["scalars"][i].data_ptr()
+        ctx = self._ctx(w, None, A, 1, 1, 0, actor, critic, mb["rnn_a"], mb["rnn_c"], 0, R, mb["actions"], mb["avail"], F)
+        ctx.stat = P(mb["stat"])
+        ctx.old_logp, ctx.old_value, ctx.returns, ctx.adv_raw, ctx.alive = (P(t) for t in mb["scalars"])
+        import ctypes
+        ga, gc = w["grads"]["actor"], w["grads"]["critic"]
+        for e in range(E):
+            for m in range(k):
+                rows = int(rows_set[e, m])
+                ga.zero_(); gc.zero_(); w["SM"].zero_()
+                if rows > 0:        # a rank that holds no row of this set adds zero gradients to the all-reduce
+                    self._mark("gather")
+                    sel = src_rows[e, m] if rows == cap else src_rows[e, m, :, :rows].contiguous()
+                    g.idx, g.rows_dst = P(sel), rows
+                    _lib.check(lib.iplan_learner_gather_rows(ctypes.byref(g), st), "gather_rows")
+                    ctx.n_eps, ctx.rnn_stride_agent = rows, rows * R
+                    ctx.norm, ctx.train_rows = P(norm_sets[e, m]), P(count_sets[e, m])
+                    self._forward(w, ctx, None, A, rows, Fp, F, actor, critic, train=True, src=mb)
+                    self._mark("fc1_bwd")
+                    _lib.check(lib.iplan_learner_fc1_backward(
+                        P(actor), self.stacks["actor"].stride(), P(critic), self.stacks["critic"].stride(),
+                        P(ga), P(gc), P(mb["Xh"]), P(mb["Xl"]), rows * Fp, Fp, F, rows, A,
+                        P(w["Z1"]), P(w["Dh"]), P(w["Dl"]), P(w["gscale"]), P(w["SM"]), P(w["G"]), st), "fc1_backward")
+                self._mark("allreduce")
+                if dist:
+                    self.bucket.allreduce([ga, gc])      # ONE NCCL all-reduce per mini-batch
+                self._mark("adam")
+                for kind, gr, col in (("actor", ga, 4), ("critic", gc, 5)):
+                    self.steps[kind] += 1
+                    stack = self.stacks[kind]
+                    _lib.check(lib.iplan_learner_adam(
+                        P(stack.flat), P(gr), P(self.exp_avg[kind]), P(self.exp_avg_sq[kind]),
+                        P(self.masks[kind]), P(w["sq"]), stack.stride(), stack.total, A,
+                        self.lrs[kind], 0.9, 0.999, self.optim_eps, self.steps[kind], self.max_grad_norm,
+                        self.grad_scale, P(w["stats"]), col, st), "adam")
+
+    def generate_data(self, obs, rnn_states_actor, rnn_states_critic, actions, returns, terminated, action_log_probs,
+                      advantages, available_actions, value_preds, num_mini_batch=None, mini_batch_size=None, perm=None):
+        """Reference :368-424: yields, per mini-batch, the ten row-indexed tensors (obs, actor / critic hidden inputs,
+        actions, value predictions, returns, alive masks, old log-probs, advantages, available actions) of one
+        permutation of the batch_size * episode_limit training rows.  ``perm`` gives the permutation; by default it is
+        drawn from the generator train() draws from.  Like the reference, ``available_actions`` loses its last episode
+        before it is flattened, which is consistent with the row indices when batch_size < buffer_size."""
+        n = self.batch_size * self.episode_limit
+        if mini_batch_size is None:
+            assert n >= num_mini_batch, f"batch_size * episode_limit = {n} rows cannot fill {num_mini_batch} mini-batches"
+            mini_batch_size = n // num_mini_batch
+        if perm is None:
+            perm = th.randperm(n, generator=self.perm_gen)
+        perm = th.as_tensor(perm).long().to(self.device)
+        flat = lambda x, last=None: x.to(self.device).reshape(-1, x.shape[-1] if last is None else last)
+        obs, rnn_states_actor, rnn_states_critic = flat(obs), flat(rnn_states_actor), flat(rnn_states_critic)
+        actions, action_log_probs = flat(actions), flat(action_log_probs)
+        if available_actions is not None:
+            available_actions = flat(available_actions[:-1])
+        value_preds, returns, terminated = flat(value_preds, 1), flat(returns, 1), flat(terminated, 1)
+        advantages = flat(advantages, 1) if advantages is not None else None
+        for i in range(num_mini_batch):
+            ind = perm[i * mini_batch_size:(i + 1) * mini_batch_size]
+            yield (obs[ind], rnn_states_actor[ind], rnn_states_critic[ind], actions[ind], value_preds[ind], returns[ind],
+                   terminated[ind], action_log_probs[ind], advantages[ind] if advantages is not None else None,
+                   available_actions[ind] if available_actions is not None else None)
 
     # ---- reference-named helper (reference :344-365) ------------------------------------
     def compute_returns(self, agent_id, obs_all, rewards, terminated, rnn_state_critic_all):

@@ -24,6 +24,31 @@ def shard_train_episodes(rank, world, eps_local, batch_size_global):
     return int(max(0, min(eps_local, batch_size_global - rank * eps_local)))
 
 
+def local_minibatch_rows(perm, num_mini_batch, T, ep_lo, ep_hi):
+    """A rank's share of the shuffled mini-batches (num_mini_batch > 1; generate_data, learners/ippo_learner.py:368-424).
+
+    ``perm`` [..., n] holds global permutations of the training rows r = b * T + t (b a global episode, rank-major).
+    Set m of a permutation is perm[m * mbs : (m + 1) * mbs], mbs = n // num_mini_batch; the n % num_mini_batch
+    trailing entries belong to no set.  The rank that holds the training episodes [ep_lo, ep_hi) keeps, per set and in
+    the permutation's order, the rows of its own episodes, renumbered (b - ep_lo) * T + t.
+
+    Returns ``idx`` [..., num_mini_batch, cap] (cap = the rank's largest share of a set; shorter shares are padded with
+    -1) and ``count`` [..., num_mini_batch].  Over the ranks the shares of a set add up to the set, whatever the sizes."""
+    n = perm.shape[-1]
+    mbs = n // num_mini_batch
+    sets = perm[..., :num_mini_batch * mbs].reshape(*perm.shape[:-1], num_mini_batch, mbs).long()
+    ep = sets // T
+    mine = (ep >= ep_lo) & (ep < ep_hi)
+    count = mine.sum(-1)
+    cap = int(count.max()) if count.numel() else 0
+    if cap == mbs and bool(mine.all()):
+        return sets - ep_lo * T, count
+    order = torch.argsort((~mine).to(torch.uint8), dim=-1, stable=True)[..., :cap]      # own rows first, order kept
+    idx = torch.gather(sets - ep_lo * T, -1, order)
+    pad = torch.arange(cap, device=perm.device) >= count.unsqueeze(-1)
+    return idx.masked_fill(pad, -1), count
+
+
 def allreduce_sum_(t):
     """In-place SUM all-reduce when a process group with >1 rank is active; no-op otherwise."""
     d = dist_or_none()
